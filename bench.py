@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- edges/sec of the KGE training hot path (BASELINE.json metric) on N B200s.
+"""bench.py -- edges/sec of the KGE training hot path (BASELINE.json metric) on N H100s.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run)
   python bench.py --impl reference --gpus N --steps K --warmup W
+  python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR   (also writes the last timed step's results as .npy)
 
 A "step" is one pass of the hot path (gather -> score over 1 positive + chunk-shared negatives ->
 logsigmoid/self-adversarial loss gradient -> row-sparse Adagrad) over one batch of B synthetic edges.
@@ -17,7 +18,6 @@ import json
 import os
 import subprocess
 import sys
-import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
@@ -27,22 +27,23 @@ for _p in (ROOT, os.path.join(ROOT, "dgl-ke_b200")):
 
 WORKLOADS = {
     # name: (model, n_ent, n_rel, hidden, gamma, lr, rc, neg, double_ent, default batch, description)
-    # default batch 14800 = 74 chunks of 200: the contraction GEMMs then launch 148 / 296 CTAs = whole waves of the 148 SMs
-    "fb15k_transe_l2": ("TransE_l2", 14951, 1345, 400, 19.9, 0.25, 1e-9, 200, False, 14800,
+    # default batch 13200 = 66 chunks of 200: each fused kernel then runs 132 (chunk, 128-row tile) work items = one wave of
+    # the H100's 132 SMs
+    "fb15k_transe_l2": ("TransE_l2", 14951, 1345, 400, 19.9, 0.25, 1e-9, 200, False, 13200,
                         "TransE_l2 FB15k-shape d=400 neg=200 -adv (BASELINE configs[1])"),
     "wikikg2_rotate": ("RotatE", 2500604, 535, 200, 12.0, 0.01, 1e-9, 256, True, 4096,
                        "RotatE wikikg2-shape d=200 -de neg=256 -adv (BASELINE configs[2])"),
-    "freebase_complex": ("ComplEx", 86054151, 14824, 400, 143.0, 0.1, 2e-6, 200, False, 14800,
-                         "ComplEx Freebase-shape 86M entities d=400 neg=200 -adv (BASELINE configs[3])"),
+    "freebase_complex": ("ComplEx", 86054151, 14824, 400, 143.0, 0.1, 2e-6, 200, False, 13200,
+                         "ComplEx Freebase-shape 86M entities d=400 neg=200 -adv (BASELINE configs[3]); 137.7 GB: sharded over >= 2 GPUs"),
     "synth_distmult": ("DistMult", 100000000, 10000, 512, 143.0, 0.08, 2e-6, 1024, False, 4096,
-                       "DistMult synthetic 100M entities d=512 neg=1024 -adv (BASELINE configs[4])"),
-    "freebase_transe_l2": ("TransE_l2", 86054151, 14824, 400, 19.9, 0.25, 1e-9, 200, False, 14800,
+                       "DistMult synthetic 100M entities d=512 neg=1024 -adv (BASELINE configs[4]); 204.8 GB: sharded over >= 4 GPUs"),
+    "freebase_transe_l2": ("TransE_l2", 86054151, 14824, 400, 19.9, 0.25, 1e-9, 200, False, 13200,
                            "TransE_l2 d=400 neg=200 -adv on the Freebase-shaped table (86 M entities, 137.7 GB; 14 824 relations): "
-                           "north_star's multi-GPU scaling shape, HBM-resident"),
-    "big_transe_l2": ("TransE_l2", 20000000, 1345, 400, 19.9, 0.25, 1e-9, 200, False, 14800,
-                      "TransE_l2 d=400 neg=200 -adv on a 20M-entity (32 GB) table: HBM-resident variant of configs[1]"),
+                           "the multi-GPU scaling shape, HBM-resident when sharded over >= 2 GPUs of 80 GB"),
+    "big_transe_l2": ("TransE_l2", 20000000, 1345, 400, 19.9, 0.25, 1e-9, 200, False, 13200,
+                      "TransE_l2 d=400 neg=200 -adv on a 20M-entity (32 GB) table: HBM-resident variant of configs[1] that fits one 80 GB GPU"),
 }
-METRIC = "edges/sec TransE_l2 d=400 neg=200 at 1/2/4/8 B200 vs ref CPU; HBM GB/s %peak"
+METRIC = "edges/sec TransE_l2 d=400 neg=200 at 1/2/4/8 H100 vs ref CPU; HBM GB/s %peak"
 
 
 def bytes_per_edge(de, dr):
@@ -57,8 +58,9 @@ def parse():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default=None, choices=sorted(WORKLOADS),
-                    help="default: fb15k_transe_l2 (BASELINE configs[1]) on one GPU, freebase_transe_l2 (the 86 M-entity "
-                         "HBM-resident table north_star's scaling target names) on several; the other one is measured beside it")
+                    help="default: fb15k_transe_l2 (BASELINE configs[1]) on one GPU with big_transe_l2 (a 32 GB table, far beyond "
+                         "L2) measured beside it; freebase_transe_l2 (the 86 M-entity table, sharded) on several GPUs with "
+                         "fb15k_transe_l2 beside it")
     ap.add_argument("--edge-placement", default="head-owner", choices=["head-owner", "random"],
                     help="N>1: which edges a rank trains on -- those whose head row it owns (half of the positive-node rows "
                          "are then local), or any (every row remote with probability (N-1)/N)")
@@ -67,12 +69,17 @@ def parse():
     ap.add_argument("--no-beside", action="store_true", help="skip the second (beside) workload of a default run")
     ap.add_argument("--batch", type=int, default=0, help="edges per step per GPU (0 = workload default)")
     ap.add_argument("--n-ent", type=int, default=0, help="override the entity count (capacity experiments)")
-    ap.add_argument("--engine", type=int, default=-1, help="-1 library default, 0 fp32 tiles, 1 tcgen05")
+    ap.add_argument("--engine", type=int, default=-1, help="-1 library default, 0 fp32 tiles, 1 wgmma")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="time eager launches instead of CUDA graphs (profiling)")
     ap.add_argument("--no-flush", action="store_true", help="do not flush L2 between timed steps")
-    ap.add_argument("--cpu-procs", type=int, default=16, help="reference arm: Hogwild worker processes (default 16, capped by the host's cores: the fastest count on the 128-vCPU GPU hosts, pinned so that the GPU/CPU ratio does not move with a probe; 0 = probe 8/16/32/64/all and use the fastest)")
-    ap.add_argument("--cpu-impl", default="auto", choices=["auto", "reference", "port"], help="reference arm: the unmodified reference installed under baseline/_ref, or the oracle port")
+    ap.add_argument("--cpu-procs", type=int, default=16, help="reference arm: Hogwild worker processes (default 16, capped by the host's cores; pinned so that the GPU/CPU ratio does not move with a probe; 0 = probe 8/16/32/64/all and use the fastest)")
+    ap.add_argument("--cpu-impl", default="auto", choices=["auto", "reference", "port"], help="reference arm: the unmodified reference installed under oracle/_ref, or the oracle port")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned and updated -- its log scalars and, on "
+                         "one GPU, the entity / relation tables with their Adagrad state (for a large table a fixed seeded sample "
+                         "of the rows that step touched) -- as DIR/<name>.npy; the inputs are seeded, so two builds can be "
+                         "compared output for output")
     ap.add_argument("--cpu-batch", type=int, default=1000, help="reference arm: batch per worker (dglke_train's 1000)")
     return ap.parse_args()
 
@@ -107,8 +114,8 @@ def run_reference(args):
     if impl == "auto":
         impl = "reference" if cpu_bench.reference_installed() else "port"
     # Hogwild workers contend on the shared tables (FB15k has only 15k entity rows), so more workers is not
-    # monotonically faster -- on the 128-vCPU GPU-box hosts 16 workers reach ~3x the throughput of 128.  The count is
-    # pinned (--cpu-procs, default 16); --cpu-procs 0 probes a few counts briefly and times the best one.
+    # monotonically faster.  The count is pinned (--cpu-procs, default 16); --cpu-procs 0 probes a few counts briefly
+    # and times the best one.
     cands = [min(args.cpu_procs, ncpu)] if args.cpu_procs else sorted({c for c in (8, 16, 32, 64, ncpu) if c <= ncpu} or {ncpu})
     probe = {}
     if len(cands) > 1:
@@ -124,7 +131,7 @@ def run_reference(args):
         "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": desc, "batch_per_worker": B, "workers": nproc,
                    "entities": n_ent_cpu, "entities_scaled_down": scaled,
-                   "note": ("the UNMODIFIED reference (baseline/_ref: KEModel.forward -> loss.backward() -> update, dgl stubbed) "
+                   "note": ("the UNMODIFIED reference (oracle/_ref: KEModel.forward -> loss.backward() -> update, dgl stubbed) "
                             if impl == "reference" else "oracle port of the reference's PyTorch step (oracle/kge_oracle.py) ") +
                            "under dglke_train's process model: Hogwild workers on shared-memory tables, 1 thread each; sampling excluded"},
         "cpu_baseline": {"value": eps, "unit": "edges/s", "cores": nproc, "kind": impl,
@@ -143,6 +150,7 @@ class ClockSampler:
          "clocks_event_reasons.sw_power_cap")
 
     def __init__(self, gpu_index):
+        import tempfile
         self.f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
         self.p = None
         try:
@@ -222,14 +230,14 @@ def run_ours(args):
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
-        # (the relation all-reduce runs beside the cooperative update kernel, which leaves it 16 SMs; capping NCCL with
-        # NCCL_MAX_CTAS=16 was measured SLOWER at 2 GPUs -- the cap is left to the environment)
+        # (the relation all-reduce runs beside the cooperative update kernel, which leaves it 16 SMs; whether to cap NCCL
+        # with NCCL_MAX_CTAS is left to the environment)
         dist.init_process_group("nccl", device_id=dev)
     default_run = args.workload is None
     primary = args.workload or ("fb15k_transe_l2" if world == 1 else "freebase_transe_l2")
     beside = None
     if default_run and not args.no_beside and not args.batch and not args.n_ent:
-        beside = "freebase_transe_l2" if world == 1 else "fb15k_transe_l2"
+        beside = "big_transe_l2" if world == 1 else "fb15k_transe_l2"
 
     line = measure(args, primary, rank, world, local_rank, dev, cpu_base, max(1, args.steps), True)
     if beside is not None:
@@ -237,9 +245,7 @@ def run_ours(args):
         other = measure(args, beside, rank, world, local_rank, dev, None, min(max(1, args.steps), 20), False)
         if rank == 0:
             line["beside"] = {k: other[k] for k in ("value", "unit", "ms_per_step", "config", "e2e", "roofline")}
-            line["beside"]["note"] = ("the same step on %s, measured in the same process: value(N) of the Freebase-shaped "
-                                      "runs against the Freebase-shaped value at N=1 is the like-for-like scaling ratio"
-                                      % WORKLOADS[beside][10])
+            line["beside"]["note"] = "the same step on %s, measured in the same process" % WORKLOADS[beside][10]
     if world > 1:
         dist.barrier()
         torch.cuda.synchronize()
@@ -250,6 +256,29 @@ def run_ours(args):
         # leave without tearing down NCCL / captured graphs / IPC mappings: destroying a process group whose
         # collectives live inside CUDA graphs has been seen to hang at exit
         os._exit(0)
+
+
+DUMP_ROWS = 16384       # rows of a large table that --dump-outputs writes (x 400 floats = 26 MB)
+
+
+def dump_outputs(out_dir, log, tables, touched):
+    """--dump-outputs: the last timed step's log scalars and, on one GPU, the tables it updated.  Of a table with more
+    than DUMP_ROWS rows, a fixed seeded sample of the rows that step touched is written (ids in <name>_rows.npy)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "log.npy"), log.detach().float().cpu().numpy())
+    if tables is None:
+        return
+    for name, emb, state, ids in (("entity", tables[0], tables[1], touched[0]), ("relation", tables[2], tables[3], touched[1])):
+        if emb.shape[0] > DUMP_ROWS:
+            ids = torch.unique(ids).cpu().numpy()
+            rows = torch.from_numpy(np.sort(np.random.default_rng(0).choice(ids, min(DUMP_ROWS, len(ids)), replace=False))).to(emb.device)
+            np.save(os.path.join(out_dir, name + "_rows.npy"), rows.cpu().numpy().astype(np.float64))
+            emb, state = emb[rows], state[rows]
+        np.save(os.path.join(out_dir, name + "_emb.npy"), emb.float().cpu().numpy())
+        np.save(os.path.join(out_dir, name + "_state.npy"), state.float().cpu().numpy())
 
 
 def measure(args, workload, rank, world, local_rank, dev, cpu_base, K_steps, full):
@@ -267,6 +296,10 @@ def measure(args, workload, rank, world, local_rank, dev, cpu_base, K_steps, ful
     hp = Hyper(model=model, hidden_dim=hidden, gamma=gamma, lr=lr, reg_coef=rc, reg_norm=3, adversarial=True,
                adv_temperature=1.0, double_ent=de)
     De, Dr = hp.entity_dim, hp.relation_dim
+    need, have = n_ent * (De + 1) * 4 // world, torch.cuda.get_device_properties(dev).total_memory
+    if need > 0.9 * have:
+        raise SystemExit("workload %s: the entity table needs %.1f GB per GPU on %d GPU(s) and this GPU has %.1f GB; use more "
+                         "GPUs (torchrun --nproc-per-node N bench.py --gpus N) or --n-ent" % (workload, need / 1e9, world, have / 1e9))
 
     # ---- tables (resident in HBM before the clock starts) ------------------------------------
     gen = torch.Generator(device=dev).manual_seed(0)
@@ -349,11 +382,11 @@ def measure(args, workload, rank, world, local_rank, dev, cpu_base, K_steps, ful
     graphs = None
     if not args.no_graph:
         try:
-            graphs = []
+            graphs, graph_logs = [], []
             for k in range(NB):
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    step_dev(k)
+                    graph_logs.append(step_dev(k))
                 graphs.append(g)
         except Exception as e:  # noqa
             sys.stderr.write("graph capture failed (%r); timing eager launches\n" % (e,))
@@ -365,6 +398,12 @@ def measure(args, workload, rank, world, local_rank, dev, cpu_base, K_steps, ful
         if int(ok.item()) == 0:
             graphs = None
 
+    last_log = [None]       # what the most recent timed step returned: its 4 log scalars (device tensor)
+
+    def replay(k):
+        graphs[k % NB].replay()
+        return graph_logs[k % NB]
+
     def timed(run_step, after=None):
         ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(K)]
         prime()
@@ -372,7 +411,7 @@ def measure(args, workload, rank, world, local_rank, dev, cpu_base, K_steps, ful
         for k in range(K):
             flush()
             ev[k][0].record()
-            run_step(k)
+            last_log[0] = run_step(k)
             if after:
                 after()
             ev[k][1].record()
@@ -385,10 +424,14 @@ def measure(args, workload, rank, world, local_rank, dev, cpu_base, K_steps, ful
 
     clk = ClockSampler(local_rank) if rank == 0 else None
     if graphs is not None:
-        ms_dev = timed(lambda k: graphs[k % NB].replay())
+        ms_dev = timed(replay)
     else:
         ms_dev = timed(step_dev)
     clocks = clk.stop() if clk else None
+    if args.dump_outputs and full and rank == 0:
+        lb = devb[(K - 1) % NB][0]           # the last timed step's batch: node ids, ..., relation ids, negative ids
+        dump_outputs(args.dump_outputs, last_log[0], (ent, ent_state, rel, rel_state) if world == 1 else None,
+                     (torch.cat([lb[0], lb[4]]), lb[3]))
 
     # launches per step, counted from one eager step
     prime()
@@ -427,27 +470,16 @@ def measure(args, workload, rank, world, local_rank, dev, cpu_base, K_steps, ful
     if rank != 0:
         return None
 
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    hbm_peak = 3350.0
+    peak_src = "data sheet: 3.35 TB/s of HBM3 on an H100 SXM (not a measured peak)"
     bpe = bytes_per_edge(De, Dr)
     edges = world * K * B
     value = edges / (ms_dev * 1e-3)
     e2e = edges / (ms_e2e * 1e-3)
     # roofline of the step's kernels: algorithmic bytes of one launch set (= one step) / summed kernel time
     achieved = B * bpe / (kern_ms * 1e-3) / 1e9 if kern_ms > 0 else 0.0
-    # DRAM traffic of one step from the committed ncu --set full capture -- only when that capture was taken on exactly
-    # this workload / batch / schedule on one GPU (profiles/summarize.py writes the key); null otherwise
+    # DRAM traffic of one step is not measured here (it needs hardware counters): null
     traffic, traffic_key = None, "%s|B=%d|launches=%d" % (workload, B, per_step_launches)
-    if world == 1:
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json"))).get(traffic_key)
-        except Exception:
-            pass
     line = {
         "metric": METRIC, "value": value, "unit": "edges/s", "n_gpus": world, "steps": K, "warmup": W,
         "ms_per_step": ms_dev / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -461,7 +493,7 @@ def measure(args, workload, rank, world, local_rank, dev, cpu_base, K_steps, ful
                                       if head_range else "random" if world > 1 else "n/a"),
                    "pipeline": ("next batch announced: its rows are fetched over NVLink by this step's fused kernels (entity reads "
                                 "lag the updates by one step, as under the reference's --async_update)") if pipelined else "none",
-                   "arithmetic": "fp32 rows; contractions on tcgen05 as 3xTF32 (hi/lo split) with fp32 accumulation" if model in ("TransE_l2", "DistMult", "ComplEx", "RESCAL") else "fp32 CUDA-core tiles",
+                   "arithmetic": "fp32 rows; contractions on wgmma as 3xTF32 (hi/lo split) with fp32 accumulation" if model in ("TransE_l2", "DistMult", "ComplEx", "RESCAL") else "fp32 CUDA-core tiles",
                    "bytes_per_edge": bpe},
         "e2e": {"value": e2e, "unit": "edges/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 16,
                 "ms_per_step": ms_e2e / K},

@@ -227,6 +227,11 @@ int carve(kge_context* h, const StepParams& p, StepWs* w, cudaStream_t stream, c
   const size_t sV = (size_t)p.B * slab_blocks(p.Ns) * 32 + 8192;
   size_t oAh = um ? take(sA) : 0, oAl = um ? take(sA) : 0, oBh = um ? take(sB) : 0, oBl = um ? take(sB) : 0;
   size_t oVh = (um && !fused) ? take(sV) : 0, oVl = (um && !fused) ? take(sV) : 0;
+  // transposed slabs: [C][rows / 32][cols][32]
+  const size_t sAT = (size_t)p.C * slab_blocks(p.Cs) * p.D * 32 + 8192, sBT = (size_t)p.C * slab_blocks(p.Ns) * p.D * 32 + 8192;
+  const size_t sVT = (size_t)p.C * slab_blocks(p.Cs) * p.Ns * 32 + 8192;
+  size_t oAhT = um ? take(sAT) : 0, oAlT = um ? take(sAT) : 0, oBhT = um ? take(sBT) : 0, oBlT = um ? take(sBT) : 0;
+  size_t oVhT = (um && !fused) ? take(sVT) : 0, oVlT = (um && !fused) ? take(sVT) : 0;
   // U-dependent tail
   size_t oNC = p.use_nc ? take(U * p.D) : 0;
   size_t oreg = take((size_t)p.B + p.Nn + (U ? (size_t)2 * p.B : 0));
@@ -257,6 +262,8 @@ int carve(kge_context* h, const StepParams& p, StepWs* w, cudaStream_t stream, c
   w->Mt = rescal ? (float*)(a + oMt) : nullptr;
   w->Ahi = at(oAh, um); w->Alo = at(oAl, um); w->Bhi = at(oBh, um); w->Blo = at(oBl, um);
   w->Vhi = at(oVh, um && !fused); w->Vlo = at(oVl, um && !fused);
+  w->AhiT = at(oAhT, um); w->AloT = at(oAlT, um); w->BhiT = at(oBhT, um); w->BloT = at(oBlT, um);
+  w->VhiT = at(oVhT, um && !fused); w->VloT = at(oVlT, um && !fused);
   return KGE_OK;
 }
 
@@ -320,7 +327,7 @@ void launch_rescal_prep_dense(const LaunchCtx&, const StepParams&, const float* 
                               const float* tail, const StepWs&, bool want_pos, bool want_a);
 void launch_rescal_chain(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
                          const BatchView&, const StepWs&);
-// tcgen05 engine (kge_umma.cu): returns false when the shape is not handled (caller falls back to engine 0)
+// wgmma engine (kge_umma.cu): returns false when the shape is not handled (caller falls back to engine 0)
 bool umma_supported(const StepParams&);
 int umma_score(const LaunchCtx&, const StepParams&, const StepWs&, char* err, size_t errlen);
 int umma_grad(const LaunchCtx&, const StepParams&, const StepWs&, bool side_b, char* err, size_t errlen);
@@ -347,8 +354,8 @@ KGE_API int kge_create(int device, kge_handle_t* out) {
   if (device < 0 || device >= n) return fail(KGE_ERR_INVALID_ARG, "device %d out of range [0,%d)", device, n);
   cudaDeviceProp prop;
   KGE_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(KGE_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major, prop.minor);
+  if (prop.major != 9)
+    return fail(KGE_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
   kge_context* h = new (std::nothrow) kge_context();
   if (!h) return fail(KGE_ERR_NOMEM, "out of host memory");
   h->device = device;
@@ -453,7 +460,7 @@ KGE_API int kge_gather(kge_handle_t h, const kge_table_t* table, const int64_t* 
 }
 
 static bool use_umma(kge_context* h, const StepParams& p) {
-  if (h->engine == 0) return false;   // engine -1 (default) / 1: tcgen05 whenever the shape allows it
+  if (h->engine == 0) return false;   // engine -1 (default) / 1: wgmma whenever the shape allows it
   return umma_supported(p);
 }
 
@@ -1046,9 +1053,8 @@ KGE_API int kge_ipc_open(kge_handle_t h, const uint8_t handle[64], int64_t offse
 
 // ---- peer-shareable shard memory (CUDA virtual memory management) --------------------------------------------------
 // A cudaMalloc range opened in another process through cudaIpcOpenMemHandle is mapped there with small pages: random
-// row reads over a 64 GB peer shard then miss the reader's TLB on every row (measured on 2 B200s, 14 800 random 1600-B
-// rows: 340 us = 70 GB/s, against 58 us when the rows are TLB-resident).  cuMemCreate allocations exported as POSIX file
-// descriptors map with 2 MiB pages on both sides (60 us cold).  tools/peer_gather_probe.py is the measurement.
+// row reads over a large peer shard then miss the reader's TLB on every row.  cuMemCreate allocations exported as POSIX file
+// descriptors map with 2 MiB pages on both sides.
 namespace {
 struct Vmm {
   CUresult (*create)(CUmemGenericAllocationHandle*, size_t, const CUmemAllocationProp*, unsigned long long) = nullptr;

@@ -1,4 +1,4 @@
-// kge_common.cuh -- shared device helpers for libkge_b200 (sm_100a only).
+// kge_common.cuh -- shared device helpers for libkge_b200 (sm_90a).
 //
 // Data model (DESIGN.md "HBM layout"):
 //   * embedding tables: fp32 row-major, row-range sharded over <= 8 GPUs (TableView); a row
@@ -52,7 +52,7 @@ struct StepParams {
   int rel_deferred;  // 1: relation Adagrad is applied later from dense all-reduced buffers (multi-GPU)
   int rel_dense;     // 1: k_chain sums relation gradients per relation into ws.rg / ws.rgs (fused single-GPU step)
   int use_nc;        // 1: head/tail rows are read from the gathered copy NC (3-call API, sharded tables); 0: from the table
-  int fused;         // 1: contraction by the fused tcgen05 kernel (kge_fused.cu): operands exist only as TF32 hi/lo slabs
+  int fused;         // 1: contraction by the fused wgmma kernel (kge_fused.cu): operands exist only as TF32 hi/lo slabs
   int hinge;         // 1: Hinge criterion (loss.py:10-17); 0: Logsigmoid == Logistic == BCE
   float margin;      // Hinge margin
   int pairwise;      // 1: criterion(pos_i - neg_ij, +1), plain mean over all (i, j) (loss.py:76-80)
@@ -97,10 +97,15 @@ struct StepWs {
   float* red_partial;         // [64 * 3] partial sums of k_reduce_log
   unsigned int* red_ticket;   // [1] completion ticket of k_reduce_log (zero between launches)
   float* Mt;       // [B, D]   RESCAL: M_r t  (tail mode needs it next to A = M_r h)
-  // tcgen05 engine: TF32 hi/lo splits of the contraction operands
+  // wgmma engine: TF32 hi/lo splits of the contraction operands
   float *Ahi, *Alo;   // [C][D/32][Cs][32]   (slab layout, see slab_off)
   float *Bhi, *Blo;   // [C][D/32][Ns][32]
   float *Vhi, *Vlo;   // [C][Ns/32][Cs][32]
+  // the same operands transposed (see slabT_off): wgmma takes TF32 operands K-major only, and the gradient GEMMs
+  // contract over the rows of these matrices
+  float *AhiT, *AloT; // [C][Cs/32][D][32]
+  float *BhiT, *BloT; // [C][Ns/32][D][32]
+  float *VhiT, *VloT; // [C][Cs/32][Ns][32]
 };
 
 struct BatchView {
@@ -204,7 +209,7 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
 __device__ __forceinline__ void split_tf32_4(float4 v, float4& h, float4& l) {
   split_tf32(v.x, h.x, l.x); split_tf32(v.y, h.y, l.y); split_tf32(v.z, h.z, l.z); split_tf32(v.w, h.w, l.w);
 }
-// tcgen05 operand layout ("k-blocked slabs"): a per-chunk matrix X[c][row][col] (row < R, col < Ncol) is stored as
+// wgmma operand layout ("k-blocked slabs"): a per-chunk matrix X[c][row][col] (row < R, col < Ncol) is stored as
 //   X[c][col / 32][row][col % 32]
 // so that every TMA box the GEMMs load -- {32 cols, n rows} of one (chunk, 32-column block) -- is ONE contiguous
 // n*128-byte region of HBM (the row-major layout made each box 128..208 scattered 128-byte lines).
@@ -212,13 +217,21 @@ __host__ __device__ inline int slab_blocks(int ncol) { return (ncol + 31) >> 5; 
 __device__ __forceinline__ long long slab_off(long long chunk, int nblk, int R, int row, int col) {
   return ((chunk * nblk + (col >> 5)) * (long long)R + row) * 32 + (col & 31);
 }
-// destination of an operand row: plain fp32 row-major and/or its TF32 hi/lo split in slab layout
+// transposed slabs: the same matrix stored as X^T[c][row / 32][col][row % 32] (Ncol rows of 32 consecutive `row`s), the
+// K-major form of X when the contraction runs over its rows
+__device__ __forceinline__ long long slabT_off(long long chunk, int R, int Ncol, int row, int col) {
+  return ((chunk * slab_blocks(R) + (row >> 5)) * (long long)Ncol + col) * 32 + (row & 31);
+}
+// destination of an operand row: plain fp32 row-major and/or its TF32 hi/lo split in slab layout (+ transposed slabs)
 struct RowOut {
   float* f32;        // row-major row pointer or null
   float* hi;         // slab-layout base pointers or null
   float* lo;
   long long chunk;
   int nblk, R, row;
+  float* hiT;        // transposed-slab base pointers or null
+  float* loT;
+  int D;             // row length (transposed slabs)
 };
 __device__ __forceinline__ void row_store4(const RowOut& o, int col, float4 v) {
   if (o.f32) *reinterpret_cast<float4*>(o.f32 + col) = v;
@@ -228,6 +241,11 @@ __device__ __forceinline__ void row_store4(const RowOut& o, int col, float4 v) {
     const long long off = slab_off(o.chunk, o.nblk, o.R, o.row, col);
     *reinterpret_cast<float4*>(o.hi + off) = h;
     *reinterpret_cast<float4*>(o.lo + off) = l;
+    if (o.hiT) {
+      const long long t = slabT_off(o.chunk, o.R, o.D, o.row, col);
+      o.hiT[t] = h.x; o.hiT[t + 32] = h.y; o.hiT[t + 64] = h.z; o.hiT[t + 96] = h.w;
+      o.loT[t] = l.x; o.loT[t + 32] = l.y; o.loT[t + 64] = l.z; o.loT[t + 96] = l.w;
+    }
   }
 }
 

@@ -1,27 +1,30 @@
-// kge_fused.cu -- the fused contraction kernel of the step (tcgen05 / TMEM / TMA, sm_100a):
+// kge_fused.cu -- the fused contraction kernel of the step (wgmma / TMA / mbarrier, sm_90a):
 //
-//   S = X . Y^T  (tensor cores, accumulator in TMEM)  ->  loss / self-adversarial softmax / backward
-//   coefficients V computed from TMEM in registers  ->  V (TF32 hi/lo) written back to TMEM
-//   ->  G = V . Y  (tensor cores, A operand read from TMEM)  ->  epilogue.
+//   S = X . Y^T  (tensor cores, accumulator in registers)  ->  loss / self-adversarial softmax / backward
+//   coefficients V computed in place in the accumulator registers  ->  G = V . Y  (tensor cores, V as the REGISTER
+//   A operand of wgmma, split into TF32 hi/lo per k-step)  ->  epilogue.
 //
 // The negative-score matrix S and the coefficient matrix V never leave the SM.  The kernel runs twice per step:
 //
-//   mode P  lanes = positives i, columns = negatives j:   S = A.Bn^T, row softmax (thread-local), GA = V.Bn
+//   mode P  rows = positives i, columns = negatives j:   S = A.Bn^T, row softmax, GA = V.Bn
 //           replaces create_neg (score_fun.py:91-108,268-286,345-376,427-449), LossGenerator.get_total_loss
 //           (loss.py:69-98) and the dL/da half of loss.backward()
-//   mode N  lanes = negatives j, columns = positives i:   S^T = Bn.A^T, V^T from the row statistics mode P left
+//   mode N  rows = negatives j, columns = positives i:   S^T = Bn.A^T, V^T from the row statistics mode P left
 //           behind, G_neg = V^T.A - colsum*b + reg'(b), mean(G_neg^2)  (the dL/db half of loss.backward() plus
 //           phase 1 of ExternalEmbedding.update for the negatives, tensor_models.py:316-328)
 //
 // Recomputing S in the second orientation costs one extra tensor-core GEMM per chunk and removes every HBM/L2 round
 // trip of S and V (and the k_loss / k_colsum / k_state_add launches).  fp32 fidelity: operands are TF32 hi/lo pairs
-// and every k-step issues hi*hi + hi*lo + lo*hi (3xTF32, fp32 accumulation in TMEM).
+// and every k-step issues hi*hi + hi*lo + lo*hi (3xTF32, fp32 accumulation).
 //
-// CTA = 384 threads: warps 0-7 epilogue (two warps per TMEM lane quarter, splitting the columns), warp 8 TMA producer,
-// warp 9 TMEM allocator + tcgen05.mma issuer (one elected lane), warps 10-11 idle (they only give their registers away).  Persistent over (chunk, 128-row tile) work
-// items.  TMEM columns: [0,N1) S -> V_hi | [N1,2N1) distances -> V_lo | [2N1, 2N1+Wc) accumulator of GEMM2, which is
-// processed in Wc-wide column chunks of the output (Wc = 96 at Ns = 200).  Shared memory: one 216 KB ring used as
-// nS1 stages {X_hi,X_lo,Y_hi,Y_lo} by GEMM1 and as nS2 stages {Y_hi,Y_lo} (MN-major) by GEMM2.
+// wgmma reads TF32 operands K-major only: GEMM1 takes the slabs of X and Y, GEMM2 the TRANSPOSED slabs of Y that
+// k_prep writes next to them (kge_common.cuh:slabT_off).
+//
+// CTA = 384 threads: warpgroups 0 and 1 (warps 0-7) each own 64 rows of the 128-row tile -- MMA issue, softmax and
+// epilogue all on the accumulator fragment, a row lives in the 4 lanes of a quad; warp 8 TMA producer, warp 9 idle (setmaxnreg acts on whole warpgroups),
+// warps 10-11 prefetch the next step's rows.  Persistent over (chunk, 128-row tile) work items.  Shared memory: one
+// 192 KB ring used as nS1 stages {X_hi,X_lo,Y_hi,Y_lo} by GEMM1 and as nS2 stages {Y^T_hi,Y^T_lo} by GEMM2, whose
+// output is produced in 128-column chunks.
 #include <cuda.h>
 #include <cstdio>
 #include <cstdlib>
@@ -35,13 +38,12 @@ using namespace tc;
 namespace {
 
 constexpr int kTileM = 128;
-constexpr int kThreadsF = 384;                    // warps 0-7 epilogue (two warpgroups), 8 TMA producer, 9 MMA issuer, 10-11 idle
-constexpr int kProducerWarp = 8, kMmaWarp = 9;
+constexpr int kThreadsF = 384;                    // warps 0-7 MMA + epilogue (two warpgroups), 8 TMA producer, 10-11 prefetch
+constexpr int kProducerWarp = 8;
 constexpr int kMaxS1 = 4, kMaxS2 = 8;
 constexpr int kMaxPf = 8;                          // row slots per prefetch warp
 constexpr uint32_t kRingBytes = 192 * 1024;
-constexpr int kStagePitch = 20;                      // floats per row of an epilogue staging tile (16 + 4 pad, 16-byte aligned rows)
-constexpr uint32_t kEpiStageBytes = 8 * 32 * kStagePitch * 4;   // one 32 x 16 tile per epilogue warp
+constexpr int kWc = 128;                           // GEMM2 output-column chunk = wgmma N
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
@@ -53,9 +55,8 @@ struct FusedArgs {
   float reg_coef;
   int reg_norm;
   int C, Rx, Ry, D;      // rows per chunk on the lane side / on the column side, row length
-  int N1;                // Ry rounded up to 16 (UMMA N of GEMM1, TMEM region width)
+  int N1;                // wgmma N of GEMM1: the kernel variant's width, >= Ry
   int nblkD;             // 32-column slab blocks of D
-  int Wc;                // GEMM2 output-column chunk (multiple of 32)
   int nS1, nS2;
   uint32_t stage1Bytes, stage2Bytes;
   const float* x2;       // |x|^2 per lane-side row   (TransE_l2)
@@ -89,56 +90,43 @@ struct FusedArgs {
   const long long* pf_neg_ids;
   float* pf_nc;                    // [nU, D] destination of the node rows (the next step's NC)
   float* pf_bn;                    // [nNeg, D] destination of the negative rows
-  unsigned long long* dbg;   // optional per-CTA timestamps of the first tile (KGE_B200_FUSED_TIMING=1)
-  int exp_halfload;          // experiment (KGE_B200_FUSED_HALFLOAD): skip the TMA loads of the lo tiles (WRONG results;
-                             // shows how much of the GEMM time is operand traffic)
 };
 
 // regulariser gradient in the epilogue: the default norm (3) inline, anything else out of line (code size: the
 // epilogue is instruction-cache sensitive)
-static __device__ __noinline__ float4 reg_grad4_any(float4 b, int norm, float coef) { return reg_grad4(b, norm, coef); }
-__device__ __forceinline__ float4 reg_grad4_fast(float4 b, int norm, float coef) {
-  if (norm == 3) {
-    const float c3 = 3.f * coef;
-    return make_float4(c3 * fabsf(b.x) * b.x, c3 * fabsf(b.y) * b.y, c3 * fabsf(b.z) * b.z, c3 * fabsf(b.w) * b.w);
-  }
-  return reg_grad4_any(b, norm, coef);
+static __device__ __noinline__ float reg_grad_any(float b, int norm, float coef) { return reg_grad(b, norm, coef); }
+__device__ __forceinline__ float reg_grad_fast(float b, int norm, float coef) {
+  if (norm == 3) return 3.f * coef * fabsf(b) * b;
+  return reg_grad_any(b, norm, coef);
 }
 
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-template <int MODE>
+template <int MODE, int NV>
 __global__ void __launch_bounds__(kThreadsF, 1)
 k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtensorMap mXl,
         const __grid_constant__ CUtensorMap mYh1, const __grid_constant__ CUtensorMap mYl1,
         const __grid_constant__ CUtensorMap mYh2, const __grid_constant__ CUtensorMap mYl2, FusedArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full1[kMaxS1], empty1[kMaxS1], full2[kMaxS2], empty2[kMaxS2];
-  __shared__ __align__(8) uint64_t s_full, v_ready, acc_full, acc_empty;
   __shared__ __align__(8) uint64_t pf_full[2][kMaxPf];
-  __shared__ uint32_t tmem_slot;
-  __shared__ __align__(16) float colA[256], colB[256], colC[256];
-  __shared__ float xch[4][2][kTileM];
-  __shared__ float rowscal[kTileM];
+  __shared__ __align__(16) float colA[NV], colB[NV], colC[NV];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint8_t* ring = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  float* epi_stage = reinterpret_cast<float*>(ring + kRingBytes);
 
   const int mtiles = (g.Rx + kTileM - 1) / kTileM;
   const int ntiles = g.C * mtiles;
   const int nkb1 = (g.D + 31) >> 5;
   const int nkb2 = (g.Ry + 31) >> 5;
-  const int nchunks = (g.D + g.Wc - 1) / g.Wc;
-  const uint32_t yBytes1 = (uint32_t)g.N1 * 128u;
-  const uint32_t yBytes2 = (uint32_t)(g.Wc >> 5) * 4096u;
-  const uint32_t colR2 = (uint32_t)g.N1, colAcc = 2u * (uint32_t)g.N1;
+  const int nchunks = (g.D + kWc - 1) / kWc;
+  constexpr uint32_t yBytes1 = (uint32_t)NV * 128u;
+  constexpr uint32_t yBytes2 = (uint32_t)kWc * 128u;
   const bool l2 = g.model == KGE_TRANSE_L2;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kMaxS1; ++s) { mbar_init(&full1[s], 1); mbar_init(&empty1[s], 1); }
-    for (int s = 0; s < kMaxS2; ++s) { mbar_init(&full2[s], 1); mbar_init(&empty2[s], 1); }
-    mbar_init(&s_full, 1); mbar_init(&v_ready, 8); mbar_init(&acc_full, 1); mbar_init(&acc_empty, 8);
+    for (int s = 0; s < kMaxS1; ++s) { mbar_init(&full1[s], 1); mbar_init(&empty1[s], 8); }
+    for (int s = 0; s < kMaxS2; ++s) { mbar_init(&full2[s], 1); mbar_init(&empty2[s], 8); }
     for (int s = 0; s < kMaxPf; ++s) { mbar_init(&pf_full[0][s], 1); mbar_init(&pf_full[1][s], 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -146,22 +134,11 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
     tma_prefetch_desc(&mXh); tma_prefetch_desc(&mXl); tma_prefetch_desc(&mYh1);
     tma_prefetch_desc(&mYl1); tma_prefetch_desc(&mYh2); tma_prefetch_desc(&mYl2);
   }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
-  if (g.dbg && threadIdx.x == 0) g.dbg[blockIdx.x * 16 + 0] = gtime();
-  (void)0;
 
-  // Roles.  The producer and MMA warps run their loops with all 32 lanes (warp-uniform control flow and operands, so the
-  // address / descriptor arithmetic stays on the uniform datapath) and one elected lane issues the TMA / tcgen05 ops.
-  // Registers: a 12-warp CTA is capped at 168 per thread; the third warpgroup (producer, MMA issuer, two idle warps)
-  // hands most of its share to the two epilogue warpgroups, which keep whole accumulator chunks and two chunks' worth of
-  // prefetched rows in registers.
+  // Roles.  The producer runs its loop with all 32 lanes (warp-uniform control flow) and one elected lane issues the
+  // TMA ops.  Registers: the third warpgroup (producer, prefetch warps) hands most of its share to the two MMA
+  // warpgroups, which keep the score accumulator and a GEMM2 accumulator chunk in registers.
   if (warp >= 8) {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
   if (warp == kProducerWarp) {
@@ -179,115 +156,33 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
         const int yx = (c * g.nblkD + kb) * g.Rx + m0;
         const int yy = (c * g.nblkD + kb) * g.Ry;
         if (elect_one()) {
-          if (g.exp_halfload) {
-            mbar_expect_tx(&full1[s], 16384u + yBytes1);
-            tma_load_2d(st, &mXh, &full1[s], 0, yx);
-            tma_load_2d(st + 32768, &mYh1, &full1[s], 0, yy);
-          } else {
           mbar_expect_tx(&full1[s], 2u * 16384u + 2u * yBytes1);
           tma_load_2d(st, &mXh, &full1[s], 0, yx);
           tma_load_2d(st + 16384, &mXl, &full1[s], 0, yx);
           tma_load_2d(st + 32768, &mYh1, &full1[s], 0, yy);
           tma_load_2d(st + 32768 + yBytes1, &mYl1, &full1[s], 0, yy);
-          }
         }
         __syncwarp();
       }
       // GEMM2 stages overlay the GEMM1 stages: wait until the tensor core has consumed all of them
       for (uint32_t k = (n1 > (uint32_t)g.nS1 ? n1 - g.nS1 : 0); k < n1; ++k) mbar_wait(&empty1[k % g.nS1], (k / g.nS1) & 1);
       for (int ch = 0; ch < nchunks; ++ch) {
-        const int d0 = ch * g.Wc;
-        int nb = (g.D - d0 + 31) >> 5;
-        if (nb > (g.Wc >> 5)) nb = g.Wc >> 5;
         for (int kb = 0; kb < nkb2; ++kb, ++n2) {
           const uint32_t s = n2 % g.nS2;
           mbar_wait(&empty2[s], ((n2 / g.nS2) & 1) ^ 1);
           uint8_t* st = ring + (size_t)s * g.stage2Bytes;
-          const int yy0 = (c * g.nblkD + (d0 >> 5)) * g.Ry + kb * 32;
+          // transposed slabs: TMA row of (chunk c, 32-row block kb of Y, column d) = (c * nblkRy + kb) * D + d
+          const int yy = (c * nkb2 + kb) * g.D + ch * kWc;
           if (elect_one()) {
-            mbar_expect_tx(&full2[s], (g.exp_halfload ? 1u : 2u) * (uint32_t)nb * 4096u);
-            for (int b = 0; b < nb; ++b) {
-              tma_load_2d(st + b * 4096, &mYh2, &full2[s], 0, yy0 + b * g.Ry);
-              if (!g.exp_halfload) tma_load_2d(st + yBytes2 + b * 4096, &mYl2, &full2[s], 0, yy0 + b * g.Ry);
-            }
+            mbar_expect_tx(&full2[s], 2u * yBytes2);
+            tma_load_2d(st, &mYh2, &full2[s], 0, yy);
+            tma_load_2d(st + yBytes2, &mYl2, &full2[s], 0, yy);
           }
           __syncwarp();
         }
       }
     }
-  } else if (warp == kMmaWarp) {
-    // ================================ MMA issuer ================================
-    uint32_t n1 = 0, n2 = 0, nacc = 0, it = 0;
-    const uint32_t idesc1 = make_idesc(kTileM, g.N1, false, false);
-    // descriptor = constant fields | (shared address >> 4): a k-step advances the address field only
-    const uint64_t descK = make_desc(0, 16, 1024), descMN = make_desc(0, 4096, 512, 1);
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      // ---- GEMM1: S = X . Y^T, K = D ----
-      for (int kb = 0; kb < nkb1; ++kb, ++n1) {
-        const uint32_t s = n1 % g.nS1;
-        mbar_wait(&full1[s], (n1 / g.nS1) & 1);
-        if (g.dbg && n1 == 0 && lane == 0) g.dbg[blockIdx.x * 16 + 1] = gtime();
-        tc_fence_after();
-        const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
-        const uint64_t dXh = descK | (uint64_t)(st >> 4), dXl = descK | (uint64_t)((st + 16384u) >> 4);
-        const uint64_t dYh = descK | (uint64_t)((st + 32768u) >> 4), dYl = descK | (uint64_t)((st + 32768u + yBytes1) >> 4);
-        const int kleft = g.D - kb * 32;
-        const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            if (ks < ksteps) {
-              const uint64_t o = (uint64_t)(ks * 2);     // K-major: +32 bytes per k-step inside the 128-byte swizzle span
-              umma_tf32(tmem_base, dXh + o, dYh + o, idesc1, (kb | ks) ? 1u : 0u);
-              umma_tf32(tmem_base, dXh + o, dYl + o, idesc1, 1u);
-              umma_tf32(tmem_base, dXl + o, dYh + o, idesc1, 1u);
-            }
-          }
-          umma_commit(&empty1[s]);
-          if (kb == nkb1 - 1) umma_commit(&s_full);
-        }
-        __syncwarp();
-      }
-      // ---- the epilogue warps turn S into V (hi | lo) in TMEM ----
-      mbar_wait(&v_ready, it & 1);
-      tc_fence_after();
-      // ---- GEMM2: G[:, chunk] = V . Y[:, chunk], K = Ry, A operand from TMEM ----
-      for (int ch = 0; ch < nchunks; ++ch, ++nacc) {
-        const int d0 = ch * g.Wc;
-        int nb = (g.D - d0 + 31) >> 5;
-        if (nb > (g.Wc >> 5)) nb = g.Wc >> 5;
-        const uint32_t idesc2 = make_idesc(kTileM, nb * 32, false, true);
-        mbar_wait(&acc_empty, (nacc & 1) ^ 1);
-        tc_fence_after();
-        for (int kb = 0; kb < nkb2; ++kb, ++n2) {
-          const uint32_t s = n2 % g.nS2;
-          mbar_wait(&full2[s], (n2 / g.nS2) & 1);
-          tc_fence_after();
-          const uint32_t st = smem_u32(ring + (size_t)s * g.stage2Bytes);
-          const uint64_t dYh = descMN | (uint64_t)(st >> 4), dYl = descMN | (uint64_t)((st + yBytes2) >> 4);
-          const uint32_t aHi = tmem_base + (uint32_t)(kb * 32), aLo = aHi + colR2;
-          const int kleft = g.Ry - kb * 32;
-          const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
-          if (elect_one()) {
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              if (ks < ksteps) {
-                // MN-major B (128B swizzle, 32B atoms): k-atoms of 4 rows (512 B, SBO), one k-step = 2 atoms = 1024 B,
-                // LBO = 4096 between the 32-wide column blocks
-                const uint64_t o = (uint64_t)(ks * 64);
-                umma_tf32_ts(tmem_base + colAcc, aHi + ks * 8, dYh + o, idesc2, (kb | ks) ? 1u : 0u);
-                umma_tf32_ts(tmem_base + colAcc, aHi + ks * 8, dYl + o, idesc2, 1u);
-                umma_tf32_ts(tmem_base + colAcc, aLo + ks * 8, dYh + o, idesc2, 1u);
-              }
-            }
-            umma_commit(&empty2[s]);
-            if (kb == nkb2 - 1) umma_commit(&acc_full);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (g.pf_slots > 0) {
+  } else if (warp >= 10 && g.pf_slots > 0) {
     // ================================ prefetch warps 10, 11 ================================
     // Each warp streams table rows (peer memory when the table is sharded) through a few shared-memory slots into the
     // next step's buffers: bulk load -> mbarrier -> bulk store, S slots per warp re-used round robin.  The loop is warp-uniform (one
@@ -321,8 +216,8 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
     };
     for (long long k = 0; k < n && k < S; ++k) load(k);
     // A slot is re-loaded L stores after its own store was issued (S - L loads in flight).  L = 1 keeps the most loads in
-    // flight, which is what matters when the rows are remote (8 GPUs: ~4 us per row); a larger L (KGE_B200_PF_LAG) never
-    // waits on the copy engine's queue for the newest store -- measured equal at 2 GPUs.
+    // flight, which is what matters when the rows are remote; a larger L (KGE_B200_PF_LAG) never waits on the copy
+    // engine's queue for the newest store.
     const int L = g.pf_lag < S - 1 ? g.pf_lag : (S > 2 ? S - 2 : 1);
     for (long long k = 0; k < n; ++k) {
       const int s = (int)(k % S);
@@ -345,396 +240,319 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
     __syncwarp();
   }
   } else {
-    // ================================ epilogue warps 0..7 ================================
+    // ================================ MMA + epilogue warps 0..7 ================================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
-    const int ehalf = warp >> 2;                  // two warps share a quarter and split the columns
-    const int row = q * 32 + lane;                // accumulator row = lane-side row inside the tile
+    const int wg = warp >> 2, q = lane & 3;
     const int et = threadIdx.x;                   // 0..255
-    const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16);
-    const int h0 = ((g.N1 >> 1) + 15) & ~15;
-    const int cb = ehalf ? h0 : 0, ce = ehalf ? g.N1 : h0;
-    uint32_t nacc = 0, it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread's rows inside the tile: rloc, rloc + 8
+    uint32_t n1 = 0, n2 = 0;
+    float acc[NV / 2];                            // S -> V: rows rloc (+8), columns 8 j + 2 q + {0, 1}
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const int c = tile / mtiles, m0 = (tile % mtiles) * kTileM;
-      const int m = m0 + row;
-      const bool row_ok = m < g.Rx;
-      const long long gx = (long long)c * g.Rx + m;
       epi_bar();                                  // everybody is done with the previous tile's shared constants
-      for (int y = et; y < g.N1; y += 256) {
+      for (int y = et; y < NV; y += 256) {
         const bool ok = y < g.Ry;
         const long long gy = (long long)c * g.Ry + y;
         colA[y] = (l2 && ok) ? g.y2[gy] : 0.f;
         if (MODE == F_N) { colB[y] = ok ? g.cstat_m[gy] : 0.f; colC[y] = ok ? g.cstat_k[gy] : 0.f; }
       }
       epi_bar();
-      const float x2v = (l2 && row_ok) ? g.x2[gx] : 0.f;
-      float colsum = 0.f;
-      // mode N, one GPU: table rows of the 4 lane-side rows this lane handles in the transposed epilogue mapping
-      // (ids fetched now, while GEMM1 runs: the epilogue's row loads then depend on nothing)
-      const float* brow[4] = {nullptr, nullptr, nullptr, nullptr};
-      const bool bdirect = MODE == F_N && (g.xids || g.xraw);
-      if (bdirect) {
+      // ---- GEMM1: S = X . Y^T, K = D ----
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          const int mr = m0 + q * 32 + (lane >> 2) + 8 * it;
-          const long long xr = (long long)c * g.Rx + (mr < g.Rx ? mr : 0);
-          brow[it] = g.xraw ? g.xraw + xr * (long long)g.D : row_ptr(g.xtab, g.xids[xr]);
+      for (int i = 0; i < NV / 2; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < nkb1; ++kb, ++n1) {
+        const uint32_t s = n1 % g.nS1;
+        mbar_wait(&full1[s], (n1 / g.nS1) & 1);
+        const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
+        const uint64_t dXh = make_desc(st + wg * 8192u), dXl = make_desc(st + 16384u + wg * 8192u);
+        const uint64_t dYh = make_desc(st + 32768u), dYl = make_desc(st + 32768u + yBytes1);
+        const int kleft = g.D - kb * 32;
+        const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
+        wgmma_fence();
+        for (int ks = 0; ks < ksteps; ++ks) {
+          const uint64_t o = (uint64_t)(ks * 2);     // K-major: +32 bytes per k-step inside the 128-byte swizzle span
+          wgmma_ss<NV>(acc, dXh + o, dYh + o, 1u);
+          wgmma_ss<NV>(acc, dXh + o, dYl + o, 1u);
+          wgmma_ss<NV>(acc, dXl + o, dYh + o, 1u);
+        }
+        wgmma_commit();
+        if (kb > 0) {
+          wgmma_wait<1>();                           // the previous k-block has retired: its stage is free
+          if (lane == 0) mbar_arrive(&empty1[(n1 - 1) % g.nS1]);
         }
       }
-      mbar_wait(&s_full, it & 1);
-      tc_fence_after();
-      const bool probe = g.dbg && it == 0 && threadIdx.x == 0;
-      if (probe) g.dbg[blockIdx.x * 16 + 2] = gtime();
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(&empty1[(n1 - 1) % g.nS1]);
+      reg_fence(acc);
 
-      float rscale = 1.f;          // mode P: 1 / softmax denominator, applied to the rows of GA in the GEMM2 epilogue
-      if (MODE == F_P) {
-        const float w_i = (g.wt && row_ok) ? g.wt[gx] : 1.f;
-        const float kw = w_i * g.inv2B;
-        // ---- pass A: scores (distance epilogue for TransE_l2), running max; 1/dist parked in TMEM region 2 ----
-        float mxl = -INFINITY;
-        if (l2 || g.adversarial || g.dumpS) {
-          for (int col = cb; col < ce; col += 16) {
-            float v[16], rr[16];
-            tmem_ld16(trow + col, v);
+      // ---- S -> V in place, two rows per thread; a row's statistics are reduced over the 4 lanes of its quad ----
+      float rscal[2];                             // mode P: 1 / softmax denominator; mode N: colsum (TransE_l2)
 #pragma unroll
-            for (int e = 0; e < 16; ++e) {
-              float s = v[e];
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + rloc + 8 * h;
+        const bool row_ok = m < g.Rx;
+        const long long gx = (long long)c * g.Rx + (row_ok ? m : 0);
+        const float x2v = (l2 && row_ok) ? g.x2[gx] : 0.f;
+        if (MODE == F_P) {
+          const float w_i = (g.wt && row_ok) ? g.wt[gx] : 1.f;
+          const float kw = w_i * g.inv2B;
+          // ---- pass A: scores (distance epilogue for TransE_l2), running max ----
+          float mxl = -INFINITY;
+          if (g.adversarial || g.dumpS) {
+#pragma unroll
+            for (int j = 0; j < NV / 8; ++j) {
+              float sv[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int col = 8 * j + 2 * q + e;
+                float s = acc[4 * j + 2 * h + e];
+                if (l2) {
+                  // batched_l2_dist (score_fun.py:26-34): (|b|^2 - 2 a.b) + |a|^2, clamp 1e-30, sqrt
+                  const float sqc = fmaxf(fmaf(-2.f, s, colA[col]) + x2v, 1e-30f);
+                  s = g.gamma - sqc * rsqrta(sqc);
+                }
+                sv[e] = s;
+                if (col < g.Ry) mxl = fmaxf(mxl, s * g.Tl2e);
+              }
+              if (g.dumpS && row_ok && 8 * j + 2 * q < g.Ry)
+                *reinterpret_cast<float2*>(g.dumpS + gx * g.Ry + 8 * j + 2 * q) = make_float2(sv[0], sv[1]);
+            }
+          }
+          if (g.adversarial) {
+            mxl = fmaxf(mxl, __shfl_xor_sync(0xffffffffu, mxl, 1));
+            mxl = fmaxf(mxl, __shfl_xor_sync(0xffffffffu, mxl, 2));
+          } else {
+            mxl = 0.f;
+          }
+          // ---- pass C: softmax numerators, loss terms and (unnormalised) backward coefficients.  The 1/denominator of
+          //      the row is a per-row scalar: it is applied to the loss sums here and to the row of GA in the GEMM2
+          //      epilogue. ----
+          float nls = 0.f, rs = 0.f, den = 0.f;
+#pragma unroll
+          for (int j = 0; j < NV / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = 8 * j + 2 * q + e;
+              float s = acc[4 * j + 2 * h + e], rinv = 1.f;
               if (l2) {
-                // batched_l2_dist (score_fun.py:26-34): (|b|^2 - 2 a.b) + |a|^2, clamp 1e-30, sqrt
-                const float sq = fmaf(-2.f, v[e], colA[col + e]) + x2v;
+                const float sq = fmaf(-2.f, s, colA[col]) + x2v;
                 const float sqc = fmaxf(sq, 1e-30f);
                 const float r = rsqrta(sqc);
                 s = g.gamma - sqc * r;
-                rr[e] = (sq > 1e-30f) ? r : 0.f;        // clamped distance: zero gradient (clamp_min_), dist ~ 0
-                v[e] = s;
+                rinv = (sq > 1e-30f) ? r : 0.f;        // clamped distance: zero gradient (clamp_min_), dist ~ 0
               }
-              if (col + e < g.Ry) mxl = fmaxf(mxl, s * g.Tl2e);
+              const float pe = g.adversarial ? ex2a(fmaf(s, g.Tl2e, -mxl)) : 1.f;
+              const float t = ex2a(-fabsf(s) * kLog2e);
+              const float u = 1.f + t;
+              const float r1 = rcpa(u);
+              const float sig = (s >= 0.f) ? r1 : t * r1;                     // sigmoid(s)
+              const float sp = fmaf(kLn2, lg2a(u), fmaxf(s, 0.f));            // -logsigmoid(-s)
+              const bool ok = row_ok && (col < g.Ry);
+              const float coef = ok ? pe * sig * kw * rinv : 0.f;              // dL/dneg_ij (/ dist) * denominator
+              if (ok) { nls = fmaf(pe, sp, nls); den += pe; }
+              rs += coef;
+              acc[4 * j + 2 * h + e] = coef;
             }
-            if (g.dumpS && row_ok) {
-#pragma unroll
-              for (int q4 = 0; q4 < 4; ++q4)
-                if (col + q4 * 4 < g.Ry) st4(g.dumpS + gx * g.Ry + col + q4 * 4, make_float4(v[q4 * 4], v[q4 * 4 + 1], v[q4 * 4 + 2], v[q4 * 4 + 3]));
-            }
-            if (l2) tmem_st16(trow + colR2 + col, rr);
           }
-          if (l2) tmem_wait_st();
-        }
-        if (g.adversarial) {
-          xch[0][ehalf][row] = mxl;
-          epi_bar();
-          mxl = fmaxf(mxl, xch[0][ehalf ^ 1][row]);
+          den += __shfl_xor_sync(0xffffffffu, den, 1); den += __shfl_xor_sync(0xffffffffu, den, 2);
+          nls += __shfl_xor_sync(0xffffffffu, nls, 1); nls += __shfl_xor_sync(0xffffffffu, nls, 2);
+          rs += __shfl_xor_sync(0xffffffffu, rs, 1); rs += __shfl_xor_sync(0xffffffffu, rs, 2);
+          const float rscale = g.adversarial ? (row_ok ? 1.f / den : 0.f) : g.uni;
+          rscal[h] = rscale;
+          if (g.dumpV && row_ok) {        // test hook: the dump shows the normalised coefficients
+#pragma unroll
+            for (int j = 0; j < NV / 8; ++j)
+              if (8 * j + 2 * q < g.Ry)
+                *reinterpret_cast<float2*>(g.dumpV + gx * g.Ry + 8 * j + 2 * q) =
+                    make_float2(acc[4 * j + 2 * h] * rscale, acc[4 * j + 2 * h + 1] * rscale);
+          }
+          if (q == 0 && row_ok) {
+            const float ps = g.pos[gx];
+            const float wb = g.wt ? *g.wbar : 1.f;        // loss.py:75,82: [B] * [B,1] -> mean(pl) * mean(w)
+            g.pl[gx] = softplusf(-ps);
+            g.nl[gx] = nls * rscale * w_i;
+            g.gpos[gx] = -sigmoidf(-ps) * wb * g.inv2B;
+            if (l2) g.rowsum[gx] = rs * rscale;
+            g.stat_m[gx] = mxl;
+            g.stat_k[gx] = kw * rscale;
+          }
         } else {
-          mxl = 0.f;
-        }
-        // ---- pass C: softmax numerators, loss terms and (unnormalised) backward coefficients -> TMEM as TF32 hi | lo.
-        //      The 1/denominator of the row is a per-row scalar: it is applied to the loss sums here and to the row of
-        //      GA in the GEMM2 epilogue, so no separate denominator pass over TMEM is needed.
-        float nls = 0.f, rs = 0.f, den = 0.f;
-        for (int col = cb; col < ce; col += 16) {
-          float v[16], rr[16], hi[16], lo[16];
-          tmem_ld16(trow + col, v);
-          if (l2) tmem_ld16(trow + colR2 + col, rr);
+          // ---- mode N: one pass, the softmax statistics of every column (positive) come from mode P ----
+          float cs = 0.f;
 #pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            float s = v[e], rinv = 1.f;
-            if (l2) {
-              const float sqc = fmaxf(fmaf(-2.f, v[e], colA[col + e]) + x2v, 1e-30f);
-              rinv = rr[e];
-              s = g.gamma - sqc * rinv;
+          for (int j = 0; j < NV / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = 8 * j + 2 * q + e;
+              float s = acc[4 * j + 2 * h + e], rinv = 1.f;
+              if (l2) {
+                const float sq = fmaf(-2.f, s, x2v) + colA[col];
+                const float sqc = fmaxf(sq, 1e-30f);
+                const float r = rsqrta(sqc);
+                s = g.gamma - sqc * r;
+                rinv = (sq > 1e-30f) ? r : 0.f;
+              }
+              const float pe = g.adversarial ? ex2a(fmaf(s, g.Tl2e, -colB[col])) : 1.f;
+              const float t = ex2a(-fabsf(s) * kLog2e);
+              const float r1 = rcpa(1.f + t);
+              const float sig = (s >= 0.f) ? r1 : t * r1;
+              float coef = pe * colC[col] * sig * rinv;
+              if (!(row_ok && (col < g.Ry))) coef = 0.f;
+              cs += coef;
+              acc[4 * j + 2 * h + e] = coef;
             }
-            const float pe = g.adversarial ? ex2a(fmaf(s, g.Tl2e, -mxl)) : 1.f;
-            const float t = ex2a(-fabsf(s) * kLog2e);
-            const float u = 1.f + t;
-            const float r1 = rcpa(u);
-            const float sig = (s >= 0.f) ? r1 : t * r1;                     // sigmoid(s)
-            const float sp = fmaf(kLn2, lg2a(u), fmaxf(s, 0.f));            // -logsigmoid(-s)
-            const bool ok = row_ok && (col + e < g.Ry);
-            float coef = ok ? pe * sig * kw * rinv : 0.f;                    // dL/dneg_ij (/ dist) * denominator
-            if (ok) { nls = fmaf(pe, sp, nls); den += pe; }
-            rs += coef;
-            split_tf32(coef, hi[e], lo[e]);
-            v[e] = coef;
           }
+          cs += __shfl_xor_sync(0xffffffffu, cs, 1); cs += __shfl_xor_sync(0xffffffffu, cs, 2);
+          rscal[h] = cs;
           if (g.dumpV && row_ok) {
 #pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4)
-              if (col + q4 * 4 < g.Ry) st4(g.dumpV + gx * g.Ry + col + q4 * 4, make_float4(v[q4 * 4], v[q4 * 4 + 1], v[q4 * 4 + 2], v[q4 * 4 + 3]));
-          }
-          tmem_st16(trow + col, hi);
-          tmem_st16(trow + colR2 + col, lo);
-        }
-        xch[1][ehalf][row] = den;
-        xch[2][ehalf][row] = nls;
-        xch[3][ehalf][row] = rs;
-        epi_bar();
-        den += xch[1][ehalf ^ 1][row];
-        rscale = g.adversarial ? (row_ok ? 1.f / den : 0.f) : g.uni;
-        if (g.dumpV && row_ok) {        // test hook: the dump shows the normalised coefficients
-          for (int col = cb; col < ce && col < g.Ry; col += 4) {
-            float4 x = ld4(g.dumpV + gx * g.Ry + col);
-            st4(g.dumpV + gx * g.Ry + col, f4_scale(x, rscale));
+            for (int j = 0; j < NV / 8; ++j)
+              if (8 * j + 2 * q < g.Ry)
+                *reinterpret_cast<float2*>(g.dumpV + gx * g.Ry + 8 * j + 2 * q) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
           }
         }
-        if (ehalf == 0 && row_ok) {
-          nls += xch[2][1][row];
-          rs += xch[3][1][row];
-          const float ps = g.pos[gx];
-          const float wb = g.wt ? *g.wbar : 1.f;        // loss.py:75,82: [B] * [B,1] -> mean(pl) * mean(w)
-          g.pl[gx] = softplusf(-ps);
-          g.nl[gx] = nls * rscale * w_i;
-          g.gpos[gx] = -sigmoidf(-ps) * wb * g.inv2B;
-          if (l2) g.rowsum[gx] = rs * rscale;
-          g.stat_m[gx] = mxl;
-          g.stat_k[gx] = kw * rscale;
-        }
-      } else {
-        // ---- mode N: one pass, the softmax statistics of every column (positive) come from mode P ----
-        float cs = 0.f;
-        for (int col = cb; col < ce; col += 16) {
-          float v[16], hi[16], lo[16];
-          tmem_ld16(trow + col, v);
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            float s = v[e], rinv = 1.f;
-            if (l2) {
-              const float sq = fmaf(-2.f, v[e], x2v) + colA[col + e];
-              const float sqc = fmaxf(sq, 1e-30f);
-              const float r = rsqrta(sqc);
-              s = g.gamma - sqc * r;
-              rinv = (sq > 1e-30f) ? r : 0.f;
-            }
-            const float pe = g.adversarial ? ex2a(fmaf(s, g.Tl2e, -colB[col + e])) : 1.f;
-            const float t = ex2a(-fabsf(s) * kLog2e);
-            const float r1 = rcpa(1.f + t);
-            const float sig = (s >= 0.f) ? r1 : t * r1;
-            float coef = pe * colC[col + e] * sig * rinv;
-            if (!(row_ok && (col + e < g.Ry))) coef = 0.f;
-            cs += coef;
-            split_tf32(coef, hi[e], lo[e]);
-            v[e] = coef;
-          }
-          if (g.dumpV && row_ok) {
-#pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4)
-              if (col + q4 * 4 < g.Ry) st4(g.dumpV + gx * g.Ry + col + q4 * 4, make_float4(v[q4 * 4], v[q4 * 4 + 1], v[q4 * 4 + 2], v[q4 * 4 + 3]));
-          }
-          tmem_st16(trow + col, hi);
-          tmem_st16(trow + colR2 + col, lo);
-        }
-        xch[2][ehalf][row] = cs;
-        epi_bar();
-        colsum = cs + xch[2][ehalf ^ 1][row];
       }
-      // V is complete in TMEM: hand it to the MMA thread
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&v_ready);
-      if (probe) g.dbg[blockIdx.x * 16 + 3] = gtime();
-      const int tr = lane >> 2, tc4 = (lane & 3) * 4;                 // transposed mapping: rows tr + 8*it, columns tc4..tc4+3
-      const int mrow0 = m0 + q * 32;                                  // first lane-side row of this warp
-      float4 bnext[12];
-      // b values of chunk `chn` in the transposed mapping: piece pc = i / 4, rows tr + 8 * (i % 4), columns tc4..tc4+3
-      auto load_b = [&](int chn) {
-        const int d0n = chn * g.Wc;
-        int nbn = (g.D - d0n + 31) >> 5;
-        if (nbn > (g.Wc >> 5)) nbn = g.Wc >> 5;
-        const int Ncn = nbn * 32;
-        const int hcn = ((Ncn >> 1) + 15) & ~15;
-        const int cbn = ehalf ? hcn : 0, cen = ehalf ? Ncn : hcn;
-        const int npn = (cen - cbn + 15) >> 4;
+      // ---- accumulator fragment -> register A fragment of GEMM2: within every group of 8 columns a thread holds columns
+      //      2q, 2q+1 and wgmma wants k = q, q + 4 from it: exchange inside the quad.  Afterwards acc[4 j + 0..3] =
+      //      (row, k = q), (row + 8, q), (row, q + 4), (row + 8, q + 4) of k-step j. ----
+      {
+        const int srcLo = (lane & ~3) | (q >> 1), srcHi = srcLo + 2;
+        const bool odd = q & 1;
 #pragma unroll
-        for (int i = 0; i < 12; ++i) {
-          const int pc = i >> 2, it = i & 3;
-          const int k = d0n + cbn + pc * 16 + tc4, mr = mrow0 + tr + 8 * it;
-          if (chn < nchunks && pc < npn && k < g.D && mr < g.Rx) {
-            if (bdirect) {
-              bnext[i] = ld4(brow[it] + k);
-            } else {
-              const long long so = slab_off(c, g.nblkD, g.Rx, mr, k);
-              bnext[i] = f4_add(ld4(g.Xhi + so), ld4(g.Xlo + so));
-            }
-          } else {
-            bnext[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int j = 0; j < NV / 8; ++j) {
+          float o[4];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            const float a0 = __shfl_sync(0xffffffffu, v0, srcLo), a1 = __shfl_sync(0xffffffffu, v1, srcLo);
+            const float b0 = __shfl_sync(0xffffffffu, v0, srcHi), b1 = __shfl_sync(0xffffffffu, v1, srcHi);
+            o[h] = odd ? a1 : a0;
+            o[2 + h] = odd ? b1 : b0;
           }
+          acc[4 * j + 0] = o[0]; acc[4 * j + 1] = o[1]; acc[4 * j + 2] = o[2]; acc[4 * j + 3] = o[3];
         }
-      };
-      if (MODE == F_N) load_b(0);                                     // chunk 0's rows: in flight during its MMAs
+      }
 
-      // ---- GEMM2 epilogue, one output-column chunk at a time ----
-      // TMEM hands every thread one accumulator ROW; writing rows from 32 lanes touches 32 cache lines per
-      // instruction (L1 is a few KB next to the 200+ KB of shared memory, so nothing merges).  Each warp therefore
-      // transposes its 32 x 16 pieces through a private shared-memory tile: afterwards a lane owns 4 consecutive
-      // columns of 4 rows (lane / 4 + 8 * it) and a warp instruction covers 8 rows x 64 contiguous bytes.
-      float* stile = epi_stage + warp * (32 * kStagePitch);
-      // per-row scalars of this tile in the transposed mapping
-      if (ehalf == 0) rowscal[row] = (MODE == F_P) ? rscale : colsum;
-      epi_bar();
-      float rsc[4];
+      // ---- GEMM2: G[:, chunk] = V . Y[:, chunk], K = Ry, A operand from registers; epilogue per 128-column chunk ----
+      float gsq[2] = {0.f, 0.f};
+      for (int ch = 0; ch < nchunks; ++ch) {
+        const int d0 = ch * kWc;
+        float acc2[kWc / 2];
 #pragma unroll
-      for (int it = 0; it < 4; ++it) rsc[it] = rowscal[q * 32 + tr + 8 * it];
-      float gsq[4] = {0.f, 0.f, 0.f, 0.f};
-      for (int ch = 0; ch < nchunks; ++ch, ++nacc) {
-        const int d0 = ch * g.Wc;
-        int nb = (g.D - d0 + 31) >> 5;
-        if (nb > (g.Wc >> 5)) nb = g.Wc >> 5;
-        const int Nc = nb * 32;
-        const int hc = ((Nc >> 1) + 15) & ~15;
-        const int cb2 = ehalf ? hc : 0, ce2 = ehalf ? Nc : hc;
-        const int npieces = (ce2 - cb2 + 15) >> 4;
-        // mode N: the rows' own values b (for -colsum*b and the regulariser) do not depend on the accumulator.  Their
-        // loads are software-pipelined one chunk ahead (issued right after the previous chunk's accumulator was read out
-        // of TMEM), so that their latency -- microseconds while the TMA stream saturates the L2 path -- hides behind
-        // this chunk's MMAs.
-        float4 bq[12];
-        if (MODE == F_N && npieces <= 3) {
+        for (int i = 0; i < kWc / 2; ++i) acc2[i] = 0.f;
 #pragma unroll
-          for (int i = 0; i < 12; ++i) bq[i] = bnext[i];
+        for (int kb = 0; kb < (NV + 31) / 32; ++kb) {
+          if (kb >= nkb2) break;
+          const uint32_t s = n2 % g.nS2;
+          mbar_wait(&full2[s], (n2 / g.nS2) & 1);
+          const uint32_t st = smem_u32(ring + (size_t)s * g.stage2Bytes);
+          const uint64_t dYh = make_desc(st), dYl = make_desc(st + yBytes2);
+          const int kleft = g.Ry - kb * 32;
+          const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
+          // the register operands of an in-flight wgmma must stay untouched: two sets, alternating, one k-step in flight
+          // behind the one being prepared
+          uint32_t ah[2][4] = {}, al[2][4] = {};
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            const int j = kb * 4 + ks;                  // compile-time: both loops are unrolled
+            if (j < NV / 8 && ks < ksteps) {
+              if (ks >= 2) wgmma_wait<1>();
+#pragma unroll
+              for (int r = 0; r < 4; ++r) {
+                float hi, lo;
+                split_tf32(acc[4 * j + r], hi, lo);
+                ah[ks & 1][r] = __float_as_uint(hi); al[ks & 1][r] = __float_as_uint(lo);
+              }
+              wgmma_fence();
+              const uint64_t o = (uint64_t)(ks * 2);
+              wgmma_rs<kWc>(acc2, ah[ks & 1], dYh + o, 1u);
+              wgmma_rs<kWc>(acc2, ah[ks & 1], dYl + o, 1u);
+              wgmma_rs<kWc>(acc2, al[ks & 1], dYh + o, 1u);
+              wgmma_commit();
+              if (ks >= 1) { reg_fence(ah[(ks - 1) & 1]); reg_fence(al[(ks - 1) & 1]); }
+            }
+          }
+          wgmma_wait<0>();
+          reg_fence(ah[0]); reg_fence(ah[1]); reg_fence(al[0]); reg_fence(al[1]);
+          if (lane == 0) mbar_arrive(&empty2[s]);
+          ++n2;
         }
-        if (probe && ch == 1) g.dbg[blockIdx.x * 16 + 8] = gtime();          // b loads issued (and summed)
-        mbar_wait(&acc_full, nacc & 1);
-        tc_fence_after();
-        if (probe && ch == 1) g.dbg[blockIdx.x * 16 + 9] = gtime();          // accumulator of chunk 1 ready
-        if (probe && ch == 0) g.dbg[blockIdx.x * 16 + 4] = gtime();
-        if (probe && ch == nchunks - 1) g.dbg[blockIdx.x * 16 + 5] = gtime();
-        auto release = [&]() {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty);
-        };
-        // one 32-row x 16-column piece: registers (row per lane) -> tile -> (4 columns of 4 rows per lane) -> global
-        auto process_pre = [&](const uint32_t* r, int col, const int bidx) {      // rows' own values prefetched into bq[bidx..bidx+3]
-          __syncwarp();                                              // the previous piece has been read out of the tile
+        reg_fence(acc2);
+        // chunk epilogue from the fragment: rows rloc (+8), columns d0 + 8 j + 2 q + {0, 1}
 #pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4)
-            *reinterpret_cast<float4*>(stile + lane * kStagePitch + q4 * 4) =
-                make_float4(__uint_as_float(r[q4 * 4]), __uint_as_float(r[q4 * 4 + 1]), __uint_as_float(r[q4 * 4 + 2]), __uint_as_float(r[q4 * 4 + 3]));
-          __syncwarp();
-          const int k = d0 + col + tc4;
+        for (int h = 0; h < 2; ++h) {
+          const int m = m0 + rloc + 8 * h;
+          if (m >= g.Rx) continue;
+          const long long gx = (long long)c * g.Rx + m;
+          float* orow = g.out + gx * (long long)g.D;
+          const float* brow = nullptr;
+          if (MODE == F_N) brow = g.xraw ? g.xraw + gx * (long long)g.D : (g.xids ? row_ptr(g.xtab, g.xids[gx]) : nullptr);
 #pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            const int mr = mrow0 + tr + 8 * it;
-            if (k >= g.D || mr >= g.Rx) continue;
-            float4 o = *reinterpret_cast<const float4*>(stile + (tr + 8 * it) * kStagePitch + tc4);
-            if (MODE == F_P) o = f4_scale(o, rsc[it]);            // 1 / softmax denominator of the row
+          for (int j = 0; j < kWc / 8; ++j) {
+            const int k = d0 + 8 * j + 2 * q;
+            if (k >= g.D) continue;
+            float o0 = acc2[4 * j + 2 * h], o1 = acc2[4 * j + 2 * h + 1];
+            if (MODE == F_P) { o0 *= rscal[h]; o1 *= rscal[h]; }          // 1 / softmax denominator of the row
             if (MODE == F_N) {
-              float4 b;
-              b = bq[bidx + it];
-              if (l2) o = f4_fma(b, -rsc[it], o);                   // sum_i V_ij a_i - (sum_i V_ij) b_j
-              o = f4_add(o, reg_grad4_fast(b, g.reg_norm, g.reg_coef));
-              gsq[it] += f4_dot(o, o);
+              float2 b;
+              if (brow) b = *reinterpret_cast<const float2*>(brow + k);
+              else {
+                const long long so = slab_off(c, g.nblkD, g.Rx, m, k);
+                const float2 bh = *reinterpret_cast<const float2*>(g.Xhi + so), bl = *reinterpret_cast<const float2*>(g.Xlo + so);
+                b = make_float2(bh.x + bl.x, bh.y + bl.y);
+              }
+              if (l2) { o0 = fmaf(b.x, -rscal[h], o0); o1 = fmaf(b.y, -rscal[h], o1); }   // sum_i V_ij a_i - (sum_i V_ij) b_j
+              o0 += reg_grad_fast(b.x, g.reg_norm, g.reg_coef);
+              o1 += reg_grad_fast(b.y, g.reg_norm, g.reg_coef);
+              gsq[h] += o0 * o0 + o1 * o1;
             }
-            st4(g.out + ((long long)c * g.Rx + mr) * (long long)g.D + k, o);
+            *reinterpret_cast<float2*>(orow + k) = make_float2(o0, o1);
           }
-        };
-        auto process_ld = [&](const uint32_t* r, int col) {                      // wide chunks: the rows' own values are loaded here
-          __syncwarp();                                              // the previous piece has been read out of the tile
-#pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4)
-            *reinterpret_cast<float4*>(stile + lane * kStagePitch + q4 * 4) =
-                make_float4(__uint_as_float(r[q4 * 4]), __uint_as_float(r[q4 * 4 + 1]), __uint_as_float(r[q4 * 4 + 2]), __uint_as_float(r[q4 * 4 + 3]));
-          __syncwarp();
-          const int k = d0 + col + tc4;
-#pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            const int mr = mrow0 + tr + 8 * it;
-            if (k >= g.D || mr >= g.Rx) continue;
-            float4 o = *reinterpret_cast<const float4*>(stile + (tr + 8 * it) * kStagePitch + tc4);
-            if (MODE == F_P) o = f4_scale(o, rsc[it]);            // 1 / softmax denominator of the row
-            if (MODE == F_N) {
-              float4 b;
-              if (bdirect) b = ld4(brow[it] + k);
-              else { const long long so = slab_off(c, g.nblkD, g.Rx, mr, k); b = f4_add(ld4(g.Xhi + so), ld4(g.Xlo + so)); }
-              if (l2) o = f4_fma(b, -rsc[it], o);                   // sum_i V_ij a_i - (sum_i V_ij) b_j
-              o = f4_add(o, reg_grad4_fast(b, g.reg_norm, g.reg_coef));
-              gsq[it] += f4_dot(o, o);
-            }
-            st4(g.out + ((long long)c * g.Rx + mr) * (long long)g.D + k, o);
-          }
-        };
-        if (npieces <= 3) {
-          // whole half-chunk in registers: the accumulator is released before any global traffic
-          uint32_t r[48];
-#pragma unroll
-          for (int pc = 0; pc < 3; ++pc)
-            if (pc < npieces) tmem_ld16_nowait(trow + colAcc + cb2 + pc * 16, r + pc * 16);
-          tmem_wait_ld();
-          release();
-          if (MODE == F_N) load_b(ch + 1);                            // next chunk's rows, one chunk ahead
-          if (probe && ch == 1) g.dbg[blockIdx.x * 16 + 10] = gtime();       // TMEM read, accumulator released
-#pragma unroll
-          for (int pc = 0; pc < 3; ++pc)
-            if (pc < npieces) process_pre(r + pc * 16, cb2 + pc * 16, pc * 4);
-          if (probe && ch == 1) g.dbg[blockIdx.x * 16 + 11] = gtime();       // chunk 1 stored
-          if (probe && ch == 0) g.dbg[blockIdx.x * 16 + 7] = gtime();        // chunk 0 stored
-        } else {
-          for (int pc = 0; pc < npieces; ++pc) {
-            uint32_t r[16];
-            tmem_ld16_nowait(trow + colAcc + cb2 + pc * 16, r);
-            tmem_wait_ld();
-            if (pc == npieces - 1) release();
-            process_ld(r, cb2 + pc * 16);
-          }
-          if (npieces == 0) release();
         }
       }
-      if (probe) g.dbg[blockIdx.x * 16 + 6] = gtime();
       if (MODE == F_N) {
-        // mean(G_neg^2) per row: the 4 lanes that share a row, then the two warps that share the quarter
+        // mean(G_neg^2) per row: the 4 lanes that share a row
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          float v = gsq[it];
+        for (int h = 0; h < 2; ++h) {
+          float v = gsq[h];
           v += __shfl_xor_sync(0xffffffffu, v, 1);
           v += __shfl_xor_sync(0xffffffffu, v, 2);
-          if ((lane & 3) == 0) xch[3][ehalf][q * 32 + tr + 8 * it] = v;
+          const int m = m0 + rloc + 8 * h;
+          if (q == 0 && m < g.Rx) g.gsn[(long long)c * g.Rx + m] = v / (float)g.D;
         }
-        epi_bar();
-        if (ehalf == 0 && row_ok) g.gsn[gx] = (xch[3][0][row] + xch[3][1][row]) / (float)g.D;
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
   }
 }
 
-int pad16(int x) { return (x + 15) & ~15; }
 
 }  // namespace
 
-// The fused kernel keeps a whole row of the chunk's score matrix in TMEM twice (hi | lo) next to the GEMM2
-// accumulator: 2 * pad16(columns) + 32 <= 512 TMEM columns.
+// The fused kernel keeps a whole row of the chunk's score matrix in the accumulator registers of one warpgroup
+// (columns / 2 registers per thread, next to the 64 of a GEMM2 chunk): at most 240 columns.
 bool fused_supported(const StepParams& p) {
   const bool model_ok = p.model == KGE_TRANSE_L2 || p.model == KGE_DISTMULT || p.model == KGE_COMPLEX || p.model == KGE_RESCAL;
   if (!model_ok) return false;
   if (p.hinge || p.pairwise || p.neg_deg) return false;   // the fused epilogue is the plain (non-pairwise, unmasked) Logsigmoid criterion
   if ((p.D % 8) || (p.Cs % 8) || (p.Ns % 8) || p.D < 32 || p.Cs < 8 || p.Ns < 8) return false;
-  return pad16(p.Cs) <= 240 && pad16(p.Ns) <= 240;
+  return p.Cs <= 240 && p.Ns <= 240;
 }
 
 // mode 0 (P): S = A.Bn^T -> loss, coefficients -> GA;  mode 1 (N): S^T -> coefficients -> G_neg (+ mean square)
 namespace {
 // GEMM stage geometry of one mode + what the ring leaves for prefetch row slots
-struct Geometry { int Rx, Ry, N1, Wc, nS1, nS2, pf_slots; uint32_t stage1Bytes, stage2Bytes, pf_off; bool ok; };
+struct Geometry { int Rx, Ry, N1, nS1, nS2, pf_slots; uint32_t stage1Bytes, stage2Bytes, pf_off; bool ok; };
 Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
   Geometry q{};
   const bool P = mode == 0;
   q.Rx = P ? p.Cs : p.Ns; q.Ry = P ? p.Ns : p.Cs;
-  q.N1 = pad16(q.Ry);
-  int wc = (512 - 2 * q.N1) & ~31;
-  if (wc > 256) wc = 256;
-  const int dpad = (p.D + 31) & ~31;
-  if (wc > dpad) wc = dpad;
-  q.Wc = wc;
+  // wgmma's N is part of the instruction: the kernel is instantiated for these widths
+  q.N1 = q.Ry <= 64 ? 64 : (q.Ry <= 128 ? 128 : (q.Ry <= 208 ? 208 : 256));
   q.stage1Bytes = 2u * 16384u + 2u * (uint32_t)q.N1 * 128u;
-  q.stage2Bytes = 2u * (uint32_t)(wc >> 5) * 4096u;
+  q.stage2Bytes = 2u * (uint32_t)kWc * 128u;
   q.nS1 = (int)(kRingBytes / q.stage1Bytes); if (q.nS1 > kMaxS1) q.nS1 = kMaxS1;
   q.nS2 = (int)(kRingBytes / q.stage2Bytes); if (q.nS2 > kMaxS2) q.nS2 = kMaxS2;
-  q.ok = q.nS1 >= 2 && q.nS2 >= 2 && wc >= 32;
+  q.ok = q.nS1 >= 2 && q.nS2 >= 2;
   if (q.ok && want_prefetch) {
     // GEMM1 keeps its stages; GEMM2 gives up stages (never below 4) until both prefetch warps have kMaxPf row slots
     const uint32_t row = (uint32_t)p.D * 4u;
@@ -751,6 +569,30 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
   }
   return q;
 }
+
+template <int MODE, int NV>
+cudaError_t launch_variant(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+  static bool attr_set[64] = {};          // the opt-in shared-memory size is a per-device function attribute
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(k_fused<MODE, NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    attr_set[dev] = true;
+  }
+  KGE_LAUNCH_NAMED(c, MODE == F_P ? "k_fused<P: S=A.Bn^T, loss, GA=V.Bn>" : "k_fused<N: S^T, G_neg=V^T.A, mean sq>",
+                   (k_fused<MODE, NV>), grid, kThreadsF, smem, m[0], m[1], m[2], m[3], m[4], m[5], g);
+  return cudaGetLastError();
+}
+template <int MODE>
+cudaError_t launch_width(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+  switch (g.N1) {
+    case 64: return launch_variant<MODE, 64>(c, grid, smem, m, g);
+    case 128: return launch_variant<MODE, 128>(c, grid, smem, m, g);
+    case 208: return launch_variant<MODE, 208>(c, grid, smem, m, g);
+    default: return launch_variant<MODE, 256>(c, grid, smem, m, g);
+  }
+}
 }  // namespace
 
 int fused_prefetch_slots(const StepParams& p, int mode) { return geometry(p, mode, true).pf_slots; }
@@ -765,7 +607,7 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
   const bool P = mode == 0;
   const Geometry q = geometry(p, mode, pf != nullptr && ent != nullptr);
   if (!q.ok) { snprintf(err, errlen, "fused kernel: shape does not fit (N1=%d)", q.N1); return KGE_ERR_UNSUPPORTED; }
-  g.Rx = q.Rx; g.Ry = q.Ry; g.N1 = q.N1; g.Wc = q.Wc; g.nS1 = q.nS1; g.nS2 = q.nS2;
+  g.Rx = q.Rx; g.Ry = q.Ry; g.N1 = q.N1; g.nS1 = q.nS1; g.nS2 = q.nS2;
   g.stage1Bytes = q.stage1Bytes; g.stage2Bytes = q.stage2Bytes;
   if (pf && ent && q.pf_slots >= 2) {
     static const int lag_env = getenv("KGE_B200_PF_LAG") ? atoi(getenv("KGE_B200_PF_LAG")) : 1;
@@ -788,54 +630,20 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
   if (!P && w.BnRaw) g.xraw = w.BnRaw;
   g.gsn = w.gsn;
   g.out = P ? w.GA : w.Bn;
+  // GEMM2 contracts over the rows of Y: its operand is the transposed slab copy of Y
+  const float *YhT = P ? w.BhiT : w.AhiT, *YlT = P ? w.BloT : w.AloT;
   const long long rowsX = (long long)p.C * g.Rx * g.nblkD, rowsY = (long long)p.C * g.Ry * g.nblkD;
-  CUtensorMap mXh, mXl, mYh1, mYl1, mYh2, mYl2;
-  if (!tc_make_map(&mXh, Xh, rowsX, 32, kTileM, err, errlen) || !tc_make_map(&mXl, Xl, rowsX, 32, kTileM, err, errlen) ||
-      !tc_make_map(&mYh1, Yh, rowsY, 32, g.N1, err, errlen) || !tc_make_map(&mYl1, Yl, rowsY, 32, g.N1, err, errlen) ||
-      !tc_make_map(&mYh2, Yh, rowsY, 32, 32, err, errlen, true) || !tc_make_map(&mYl2, Yl, rowsY, 32, 32, err, errlen, true))
+  const long long rowsYT = (long long)p.C * slab_blocks(g.Ry) * g.D;
+  CUtensorMap m[6];
+  if (!tc_make_map(&m[0], Xh, rowsX, 32, kTileM, err, errlen) || !tc_make_map(&m[1], Xl, rowsX, 32, kTileM, err, errlen) ||
+      !tc_make_map(&m[2], Yh, rowsY, 32, g.N1, err, errlen) || !tc_make_map(&m[3], Yl, rowsY, 32, g.N1, err, errlen) ||
+      !tc_make_map(&m[4], YhT, rowsYT, 32, kWc, err, errlen) || !tc_make_map(&m[5], YlT, rowsYT, 32, kWc, err, errlen))
     return KGE_ERR_CUDA;
-  const size_t smem = kRingBytes + kEpiStageBytes + 1024;
-  static bool attr_set[2][64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[mode][dev]) {
-    cudaError_t e = P ? cudaFuncSetAttribute(k_fused<F_P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                      : cudaFuncSetAttribute(k_fused<F_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { snprintf(err, errlen, "cudaFuncSetAttribute(k_fused): %s", cudaGetErrorString(e)); return KGE_ERR_CUDA; }
-    attr_set[mode][dev] = true;
-  }
+  const size_t smem = kRingBytes + 1024;
   const int mtiles = (g.Rx + kTileM - 1) / kTileM;
   int grid = p.C * mtiles;
   if (grid > c.num_sms) grid = c.num_sms;
-  static const bool timing = getenv("KGE_B200_FUSED_TIMING") != nullptr;
-  static const bool halfload = getenv("KGE_B200_FUSED_HALFLOAD") != nullptr;
-  g.exp_halfload = halfload ? 1 : 0;
-  unsigned long long* dbg = nullptr;
-  if (timing) { cudaMalloc(&dbg, (size_t)grid * 16 * sizeof(unsigned long long)); cudaMemset(dbg, 0, (size_t)grid * 128); g.dbg = dbg; }
-  if (P) KGE_LAUNCH_NAMED(c, "k_fused<P: S=A.Bn^T, loss, GA=V.Bn>", k_fused<F_P>, grid, kThreadsF, smem, mXh, mXl, mYh1, mYl1, mYh2, mYl2, g);
-  else KGE_LAUNCH_NAMED(c, "k_fused<N: S^T, G_neg=V^T.A, mean sq>", k_fused<F_N>, grid, kThreadsF, smem, mXh, mXl, mYh1, mYl1, mYh2, mYl2, g);
-  if (timing) {
-    cudaStreamSynchronize(c.stream);
-    unsigned long long* hb = (unsigned long long*)malloc((size_t)grid * 128);
-    cudaMemcpy(hb, dbg, (size_t)grid * 128, cudaMemcpyDeviceToHost);
-    double t[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-    unsigned long long mn = ~0ull, mx = 0;
-    for (int i = 0; i < grid; ++i) {
-      const unsigned long long* r = hb + (size_t)i * 16;
-      for (int k = 1; k < 12; ++k) t[k] += (double)(r[k] - r[0]);
-      if (r[0] < mn) mn = r[0];
-      if (r[6] > mx) mx = r[6];
-    }
-    fprintf(stderr, "[fused timing] mode %c ctas=%d tiles=%d (first tile, us since CTA start) first_stage=%.2f gemm1_done=%.2f softmax_done=%.2f "
-            "gemm2_chunk0=%.2f gemm2_last=%.2f tile_end=%.2f span=%.2f  (nS1=%d nS2=%d Wc=%d N1=%d)\n"
-            "               epilogue warp 2: chunk0 stored=%.2f | chunk1: b loaded=%.2f acc ready=%.2f released=%.2f stored=%.2f\n",
-            P ? 'P' : 'N', grid, p.C * mtiles,
-            t[1] / grid / 1e3, t[2] / grid / 1e3, t[3] / grid / 1e3, t[4] / grid / 1e3, t[5] / grid / 1e3, t[6] / grid / 1e3,
-            (double)(mx - mn) / 1e3, g.nS1, g.nS2, g.Wc, g.N1,
-            t[7] / grid / 1e3, t[8] / grid / 1e3, t[9] / grid / 1e3, t[10] / grid / 1e3, t[11] / grid / 1e3);
-    free(hb); cudaFree(dbg);
-  }
-  cudaError_t e = cudaGetLastError();
+  cudaError_t e = P ? launch_width<F_P>(c, grid, smem, m, g) : launch_width<F_N>(c, grid, smem, m, g);
   if (e != cudaSuccess) { snprintf(err, errlen, "k_fused launch: %s", cudaGetErrorString(e)); return KGE_ERR_CUDA; }
   return KGE_OK;
 }

@@ -13,7 +13,7 @@
 //   k_negdeg_mask_coef    V[c, i, i] = 0 and its TF32 hi/lo copies   (after k_loss: no gradient)
 //   k_negdeg_scatter      G'[c, j] - reg'(row) is added to the positive node's gradient NG, then G'[c, j] = 0, so that the
 //                         update kernel's negative phases (state add, row scatter) see a zero gradient for those rows
-// Single-GPU tables only; the contraction takes the stand-alone GEMM / tile kernels (Ns' exceeds the fused kernel's TMEM budget
+// Single-GPU tables only; the contraction takes the stand-alone GEMM / tile kernels (Ns' exceeds the fused kernel's register budget
 // at the usual shapes, and its epilogue has no mask).
 #include "kge_common.cuh"
 
@@ -64,6 +64,9 @@ __global__ void __launch_bounds__(kBlock) k_negdeg_mask_coef(StepParams p, StepW
     const long long so = slab_off(i / p.Cs, slab_blocks(p.Ns), p.Cs, il, il);
     w.Vhi[so] = 0.f;
     w.Vlo[so] = 0.f;
+    const long long st = slabT_off(i / p.Cs, p.Cs, p.Ns, il, il);
+    w.VhiT[st] = 0.f;
+    w.VloT[st] = 0.f;
   }
 }
 

@@ -65,6 +65,10 @@ __global__ void __launch_bounds__(kBlock) k_rescal_fwd(StepParams p, const float
         split_tf32(av, hh, ll);
         const long long o = slab_off(i / p.Cs, slab_blocks(D), p.Cs, (int)(i % p.Cs), k);
         w.Ahi[o] = hh; w.Alo[o] = ll;
+        if (w.AhiT) {
+          const long long ot = slabT_off(i / p.Cs, p.Cs, D, (int)(i % p.Cs), k);
+          w.AhiT[ot] = hh; w.AloT[ot] = ll;
+        }
       }
       else w.A[i * (long long)D + k] = av;
     }

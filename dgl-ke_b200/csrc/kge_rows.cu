@@ -111,7 +111,7 @@ __device__ __forceinline__ void edge_forward(const StepParams& p, const float* _
   EdgeAcc acc{0.f, 0.f, 0.f};
   const bool reg_on = (p.reg_coef > 0.f && p.reg_norm > 0);
   // All loads of the (up to kIt) slices a lane owns are issued before any arithmetic: 9-12 independent 16-byte
-  // loads in flight per lane hide HBM latency, and the ~2 us NVLink latency when the rows live on a peer GPU.
+  // loads in flight per lane hide HBM latency, and the longer NVLink latency when the rows live on a peer GPU.
   constexpr int kIt = KIT;                                // slices per lane loaded ahead (1: local HBM, 4: sharded)
   constexpr int kItC = KIT > 1 ? KIT / 2 : 1;             // complex models load two half-rows per slice
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -191,8 +191,8 @@ __global__ void __launch_bounds__(kRowBlock) k_prep(StepParams p, TableView ent,
     const float* r = row_ptr(rel, b.rel_ids[job]);
     float pos, a2, reg, nrm;
     const long long ro = job * (long long)p.D;
-    // tcgen05 engine: A is only consumed as hi/lo operands; fp32 tiles: plain fp32
-    const RowOut ao{w.Ahi ? nullptr : w.A + ro, w.Ahi, w.Alo, job / p.Cs, slab_blocks(p.D), p.Cs, (int)(job % p.Cs)};
+    // wgmma engine: A is only consumed as hi/lo operands; fp32 tiles: plain fp32
+    const RowOut ao{w.Ahi ? nullptr : w.A + ro, w.Ahi, w.Alo, job / p.Cs, slab_blocks(p.D), p.Cs, (int)(job % p.Cs), w.AhiT, w.AloT, p.D};
     edge_forward<MODEL, KIT>(p, h, r, t, ao, lane, pos, a2, reg, nrm, true);
     if (lane == 0) {
       w.pos[job] = pos;
@@ -206,7 +206,7 @@ __global__ void __launch_bounds__(kRowBlock) k_prep(StepParams p, TableView ent,
     const long long ro = job * (long long)p.D;
     const float* src = w.BnRaw ? w.BnRaw + ro : row_ptr(ent, b.neg_ids[job]);   // staged by the previous step, or the table
     // fused contraction: the negatives exist only as TF32 hi/lo slabs (Bn receives their gradient later)
-    const RowOut bo{p.fused ? nullptr : w.Bn + ro, w.Bhi, w.Blo, job / p.Ns, slab_blocks(p.D), p.Ns, (int)(job % p.Ns)};
+    const RowOut bo{p.fused ? nullptr : w.Bn + ro, w.Bhi, w.Blo, job / p.Ns, slab_blocks(p.D), p.Ns, (int)(job % p.Ns), w.BhiT, w.BloT, p.D};
     float b2 = 0.f, reg = 0.f;
     const int nv = p.D >> 2;
     for (int v0 = 0; v0 < nv; v0 += kWarp * KIT) {
@@ -289,7 +289,7 @@ __global__ void __launch_bounds__(kRowBlock) k_prep_dense(StepParams p, const fl
     if (!want_pos) { if (p.neg_head) hrow = trow; else trow = hrow; }
     const long long ro = job * (long long)p.D;
     const RowOut ao{(want_a && !w.Ahi) ? w.A + ro : nullptr, want_a ? w.Ahi : nullptr, want_a ? w.Alo : nullptr,
-                    job / p.Cs, slab_blocks(p.D), p.Cs, (int)(job % p.Cs)};
+                    job / p.Cs, slab_blocks(p.D), p.Cs, (int)(job % p.Cs), nullptr, nullptr, p.D};
     edge_forward<MODEL, 1>(p, hrow, relr + job * (long long)p.Dr, trow, ao, lane, pos, a2, reg, nrm, want_a);
     if (lane == 0) {
       if (want_pos) w.pos[job] = pos;
@@ -301,7 +301,7 @@ __global__ void __launch_bounds__(kRowBlock) k_prep_dense(StepParams p, const fl
   if (job < p.Nn && negrows != nullptr) {
     const float* src = negrows + job * (long long)p.D;
     const long long ro = job * (long long)p.D;
-    const RowOut bo{nullptr, w.Bhi, w.Blo, job / p.Ns, slab_blocks(p.D), p.Ns, (int)(job % p.Ns)};
+    const RowOut bo{nullptr, w.Bhi, w.Blo, job / p.Ns, slab_blocks(p.D), p.Ns, (int)(job % p.Ns), nullptr, nullptr, p.D};
     float b2 = 0.f;
     for (int v = lane; v < (p.D >> 2); v += kWarp) {
       float4 x = ld4(src + 4 * v);
@@ -326,7 +326,7 @@ __global__ void __launch_bounds__(kRowBlock) k_prep_dense(StepParams p, const fl
 void launch_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
                  const BatchView& b, const StepWs& w) {
   long long jobs = p.B + p.Nn;
-  // sharded tables: deeper per-lane load batches hide the ~2 us NVLink latency; local HBM prefers occupancy
+  // sharded tables: deeper per-lane load batches hide the NVLink latency; local HBM prefers occupancy
   if (ent.n_shards > 1) {
     KGE_DISPATCH_MODEL(p.model, KGE_LAUNCH(c, (k_prep<M, 4>), ceil_div(jobs, kWarpsPerBlock), kRowBlock, 0, p, ent, rel, b, w, 0LL));
   } else {
@@ -396,7 +396,8 @@ __global__ void __launch_bounds__(kRowBlock) k_loss(StepParams p, const float* _
                                                      const float* __restrict__ wbar, float* __restrict__ V,
                                                      float* __restrict__ gpos, float* __restrict__ rowsum,
                                                      float* __restrict__ pl, float* __restrict__ nl,
-                                                     float* __restrict__ Vhi, float* __restrict__ Vlo) {
+                                                     float* __restrict__ Vhi, float* __restrict__ Vlo,
+                                                     float* __restrict__ VhiT, float* __restrict__ VloT) {
   long long i = (long long)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
   if (i >= p.B) return;
   const int lane = threadIdx.x & 31;
@@ -443,6 +444,8 @@ __global__ void __launch_bounds__(kRowBlock) k_loss(StepParams p, const float* _
         split_tf32(coef, hh, ll);
         const long long o = slab_off(chunk, nblk, p.Cs, il, j);
         Vhi[o] = hh; Vlo[o] = ll;
+        const long long ot = slabT_off(chunk, p.Cs, p.Ns, il, j);
+        VhiT[ot] = hh; VloT[ot] = ll;
       }
     }
   } else {
@@ -462,6 +465,8 @@ __global__ void __launch_bounds__(kRowBlock) k_loss(StepParams p, const float* _
         split_tf32(coef, hh, ll);
         const long long o = slab_off(chunk, nblk, p.Cs, il, j);
         Vhi[o] = hh; Vlo[o] = ll;
+        const long long ot = slabT_off(chunk, p.Cs, p.Ns, il, j);
+        VhiT[ot] = hh; VloT[ot] = ll;
       }
     }
   }
@@ -593,7 +598,7 @@ void launch_reduce_log(const LaunchCtx& c, const StepParams& p, const float* wt,
 void launch_loss_rows(const LaunchCtx& c, const StepParams& p, const float* pos, const float* S, const float* wt,
                       const StepWs& w) {
   KGE_LAUNCH(c, k_loss, ceil_div(p.B, kWarpsPerBlock), kRowBlock, 0, p, pos, S, wt, w.wbar, w.V, w.gpos, w.rowsum,
-             w.pl, w.nl, w.Vhi, w.Vlo);
+             w.pl, w.nl, w.Vhi, w.Vlo, w.VhiT, w.VloT);
 }
 
 void launch_colsum(const LaunchCtx& c, const StepParams& p, const StepWs& w) {

@@ -1,6 +1,6 @@
-// kge_tc.cuh -- inline-PTX wrappers shared by the tcgen05 kernels (kge_umma.cu, kge_fused.cu):
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05.mma (SS and TS forms) / commit / ld / st, shared-memory
-// matrix descriptors and the instruction descriptor.  sm_100a only.
+// kge_tc.cuh -- inline-PTX wrappers shared by the wgmma kernels (kge_umma.cu, kge_fused.cu):
+// mbarrier, TMA (cp.async.bulk.tensor), bulk copies, wgmma.mma_async (tf32; A from shared memory or from
+// registers) / fence / commit / wait and the shared-memory matrix descriptor.  sm_90a.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -9,14 +9,9 @@
 namespace kge {
 namespace tc {
 
-__device__ __forceinline__ unsigned long long gtime() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// exactly one lane of the (converged) warp gets true; lets ptxas keep the operands of the guarded TMA / tcgen05
+// exactly one lane of the (converged) warp gets true; lets ptxas keep the operands of the guarded TMA
 // instructions in uniform registers instead of looping over "possibly several" active lanes
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
@@ -70,86 +65,79 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-// D[tmem] (+)= A[smem] . B[smem]
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D[tmem] (+)= A[tmem] . B[smem]   (A: lane = M row, 32-bit column = K element; K-major only)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ---- wgmma (sm_90a): D[registers, 64 x N per warpgroup] (+)= A . B^T-stored-K-major, tf32 inputs, fp32 accumulation.
+// TF32 operands in shared memory are K-major only.  Accumulator fragment of thread t of the warpgroup (w = t / 32,
+// l = t % 32): d[4 j + 0..1] = row 16 w + l / 4, columns 8 j + 2 (l % 4) + {0, 1}; d[4 j + 2..3] = the same columns of
+// row + 8.  Register A fragment (one k-step of 8): a[0] = (row, k = l % 4), a[1] = (row + 8, k), a[2] = (row, k + 4),
+// a[3] = (row + 8, k + 4).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the compiler may not move uses of these registers across this point (accumulators / register operands of in-flight wgmma)
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// 16 consecutive 32-bit columns of this thread's TMEM lane; NO wait (pair with tmem_wait_ld)
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                 "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(taddr));
+__device__ __forceinline__ void reg_fence(uint32_t (&a)[4]) {
+  asm volatile("" : "+r"(a[0]), "+r"(a[1]), "+r"(a[2]), "+r"(a[3])::"memory");
 }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  tmem_ld16_nowait(taddr, r);
-  tmem_wait_ld();
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+// operand lists of the asm statements, 16 accumulator registers at a time
+#define KGE_D4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define KGE_D16(i) KGE_D4(i), KGE_D4(i + 4), KGE_D4(i + 8), KGE_D4(i + 12)
+#define KGE_D32(i) KGE_D16(i), KGE_D16(i + 16)
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_ss<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+               : KGE_D32(0)
+               : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-               ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-                 "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-                 "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])),
-                 "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-                 "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])),
-                 "r"(__float_as_uint(v[15]))
-               : "memory");
+template <>
+__device__ __forceinline__ void wgmma_ss<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
+               : KGE_D32(0), KGE_D32(32)
+               : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+template <>
+__device__ __forceinline__ void wgmma_ss<208>(float (&d)[104], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %106, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n208k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103}, %104, %105, p, 1, 1;\n\t}"
+               : KGE_D32(0), KGE_D32(32), KGE_D32(64), KGE_D4(96), KGE_D4(100)
+               : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_ss<256>(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1;\n\t}"
+               : KGE_D32(0), KGE_D32(32), KGE_D32(64), KGE_D32(96)
+               : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_rs<128>(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1;\n\t}"
+               : KGE_D32(0), KGE_D32(32)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+#undef KGE_D4
+#undef KGE_D16
+#undef KGE_D32
 
-// shared-memory matrix descriptor, 128-byte swizzle (cute::UMMA::SmemDescriptor bit layout)
-// layout_type: 2 = SWIZZLE_128B (K-major operands), 1 = SWIZZLE_128B_BASE32B (the only layout the
-// tensor core accepts for MN-major tf32 operands; matches TMA's SWIZZLE_128B_ATOM_32B)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type = 2) {
+// shared-memory matrix descriptor of a K-major tf32 tile loaded by TMA with the 128-byte swizzle: rows of 128 bytes
+// (32 floats of K), 8-row groups 1024 bytes apart (SBO); a k-step of 8 advances the start address by 32 bytes
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;            // descriptor version (Blackwell)
-  d |= (uint64_t)layout_type << 61;
-  return d;
-}
-// instruction descriptor: D=f32, A=B=tf32, majors, N>>3, M>>4 (cute::UMMA::InstrDescriptor)
-__host__ __device__ inline uint32_t make_idesc(int M, int N, bool a_mn, bool b_mn) {
-  uint32_t d = 0;
-  d |= 1u << 4;                      // c_format = F32
-  d |= 2u << 7;                      // a_format = TF32
-  d |= 2u << 10;                     // b_format = TF32
-  d |= (a_mn ? 1u : 0u) << 15;
-  d |= (b_mn ? 1u : 0u) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
+  d |= (uint64_t)1 << 16;            // LBO: unused by swizzled K-major layouts
+  d |= (uint64_t)(1024 >> 4) << 32;  // SBO
+  d |= (uint64_t)1 << 62;            // 128-byte swizzle
   return d;
 }
 
@@ -163,8 +151,7 @@ __device__ __forceinline__ float sqrta(float x) { float y; asm("sqrt.approx.ftz.
 }  // namespace tc
 
 // host side (kge_umma.cu): cached cuTensorMapEncodeTiled of a 2-D fp32 matrix [rows, cols] with box {32 cols, box_rows},
-// 128-byte swizzle (mn_major: 32-byte swizzle atoms, for MN-major tf32 operands), zero OOB fill.
-bool tc_make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen,
-                 bool mn_major = false);
+// 128-byte swizzle, zero OOB fill.
+bool tc_make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen);
 
 }  // namespace kge

@@ -1,5 +1,5 @@
 // kge_tiles.cu -- fp32 CUDA-core tile kernels for the chunked negative contraction
-// (engine 0; the tcgen05 engine in kge_umma.cu replaces the bilinear cases).
+// (engine 0; the wgmma engine in kge_umma.cu replaces the bilinear cases).
 //
 //   k_score  : S[c,i,j] = pair(a_i, b_j)                  create_neg fns, score_fun.py:26-38,91-108,
 //                                                         268-286,345-376,427-449,512-554
@@ -126,15 +126,16 @@ __global__ void __launch_bounds__(256) k_score(StepParams p, const float* __rest
 
 
 // ------------------------------------------------------------------------------------------
-// RotatE pair kernels (score_fun.py:512-554).  A complex dimension is one (re, im) float2: the pair arithmetic runs on
-// Blackwell's packed fp32x2 pipe (FADD2 / FMUL2 / FFMA2: d = a - b and d*d are one instruction each), which halves the
-// FP32 issue load of the kernels that dominate configs[2] -- what is left is one MUFU (sqrt / rsqrt) per complex pair
-// per pass, the floor of this model (SURVEY 8d: ~90 M edges/s of MUFU for the forward, a third of that with the two
-// gradient passes).
+// RotatE pair kernels (score_fun.py:512-554).  A complex dimension is one (re, im) float2; Hopper has no packed fp32x2
+// arithmetic, so the pair operations below are two scalar FADD / FMUL / FFMA each (same rounding per component), next
+// to one MUFU (sqrt / rsqrt) per complex pair per pass.
 constexpr int RT = 64;             // tile edge (rows)
 constexpr int RKS = 16;            // complex dims per slab (score)
 constexpr int RLD = RT + 2;        // float2 per smem row: 528 B, 16-byte aligned, breaks the 4-way store conflict
 
+__device__ __forceinline__ float2 pair_sub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
+__device__ __forceinline__ float2 pair_mul(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+__device__ __forceinline__ float2 pair_fma(float2 a, float s, float2 c) { return make_float2(fmaf(a.x, s, c.x), fmaf(a.y, s, c.y)); }
 __device__ __forceinline__ float sqrt_approx(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
 __global__ void __launch_bounds__(256) k_rot_score(StepParams p, const float* __restrict__ A, const float* __restrict__ Bn,
@@ -174,8 +175,8 @@ __global__ void __launch_bounds__(256) k_rot_score(StepParams p, const float* __
       for (int r = 0; r < 4; ++r)
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const float2 d = __fadd2_rn(a[r], make_float2(-b[q].x, -b[q].y));
-          const float2 sq = __fmul2_rn(d, d);
+          const float2 d = pair_sub(a[r], b[q]);
+          const float2 sq = pair_mul(d, d);
           acc[r][q] += sqrt_approx(sq.x + sq.y);       // one MUFU; ~1e-7 relative on a sum of D/2 terms
         }
     }
@@ -261,11 +262,11 @@ __global__ void __launch_bounds__(256, 4) k_rot_grad(StepParams p, const float* 
       for (int r = 0; r < 4; ++r)
 #pragma unroll
         for (int u = 0; u < KW; ++u) {
-          const float2 d = __fadd2_rn(m[r][u], make_float2(-o[u].x, -o[u].y));
-          const float2 sq = __fmul2_rn(d, d);
+          const float2 d = pair_sub(m[r][u], o[u]);
+          const float2 sq = pair_mul(d, d);
           // |d| = 0 (identical complex numbers): d itself is 0, so the finite rsqrt of the floor contributes nothing
           const float s = -vv[r] * rsqrtf(fmaxf(sq.x + sq.y, 1e-36f));
-          acc[r][u] = __ffma2_rn(d, make_float2(s, s), acc[r][u]);
+          acc[r][u] = pair_fma(d, s, acc[r][u]);
         }
     }
     __syncthreads();

@@ -1,17 +1,18 @@
-// kge_umma.cu -- tcgen05 (5th-gen tensor core) engine for the three chunked contractions of the
+// kge_umma.cu -- stand-alone wgmma (Hopper warpgroup MMA) engine (the file and its umma_* entry points keep their names) for the three chunked contractions of the
 // bilinear / L2 models (TransE_l2, DistMult, ComplEx, RESCAL):
 //
-//   GEMM1  S[c]  = A[c]   . Bn[c]^T     (Cs x Ns, K = D)    both operands K-major
-//   GEMM2  GA[c] = V[c]   . Bn[c]       (Cs x D,  K = Ns)   A K-major, B MN-major
-//   GEMM3  GB[c] = V[c]^T . A[c]        (Ns x D,  K = Cs)   both operands MN-major
+//   GEMM1  S[c]  = A[c]   . Bn[c]^T     (Cs x Ns, K = D)    operands: A, Bn slabs
+//   GEMM2  GA[c] = V[c]   . Bn[c]       (Cs x D,  K = Ns)   operands: V slabs, Bn^T slabs
+//   GEMM3  GB[c] = V[c]^T . A[c]        (Ns x D,  K = Cs)   operands: V^T slabs, A^T slabs
 //
-// fp32 fidelity on TF32 tensor cores: every operand is split x = hi + lo (both rounded to TF32) by its
-// producer (k_prep / k_loss, kge_common.cuh:split_tf32) and each k-step issues hi*hi + hi*lo + lo*hi (3xTF32), accumulating in fp32 in TMEM.
+// wgmma reads TF32 operands from shared memory K-major only, so the producers (k_prep / k_loss) write every operand in
+// both orientations (kge_common.cuh: slab_off / slabT_off) and all three GEMMs are the same K-major x K-major kernel.
+// fp32 fidelity on TF32 tensor cores: every operand is split x = hi + lo (both rounded to TF32) by its producer
+// (kge_common.cuh:split_tf32) and each k-step issues hi*hi + hi*lo + lo*hi (3xTF32), accumulating in fp32 registers.
 //
-// One CTA per 128 x Nt output tile (Nt <= 256): warp 0 = TMA producer (cp.async.bulk.tensor over the
-// contiguous slab layout, 128B swizzle, 2-stage mbarrier pipeline), warp 1 = TMEM allocator + single-thread
-// tcgen05.mma issuer, warps 2-9 = epilogue (tcgen05.ld 32x32b: one accumulator row per thread, two warps
-// per TMEM lane quarter splitting the columns).
+// One CTA per 128 x 128 output tile: warpgroups 0 and 1 each own 64 rows (wgmma m64n128k8, accumulator in registers,
+// epilogue straight from the fragments), warp 8 = TMA producer (cp.async.bulk.tensor over the contiguous slab layout,
+// 128B swizzle, 3-stage mbarrier pipeline).
 #include <cuda.h>
 #include <cstdio>
 #include <cstdlib>
@@ -25,22 +26,20 @@ using namespace tc;
 namespace {
 
 constexpr int kBlockK = 32;                 // fp32 elements per k-block = one 128-byte swizzle span
-constexpr int kUmmaK = 8;                   // tf32: 32 bytes per MMA k-step
-constexpr int kTileM = 128;
-constexpr int kStages = 2;
-constexpr int kThreads = 320;                // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quarter)
-constexpr int kTmemCols = 256;
+constexpr int kMmaK = 8;                    // tf32: 32 bytes per MMA k-step
+constexpr int kTileM = 128, kTileN = 128;
+constexpr int kStages = 3;
+constexpr int kThreads = 384;                // warps 0..7 MMA + epilogue (two warpgroups), warp 8 TMA producer
+constexpr uint32_t kTileBytes = 128 * 128;   // one operand tile (hi or lo): 128 rows x 128 B
+constexpr uint32_t kStageBytes = 4 * kTileBytes;
 
 enum { G_SCORE = 0, G_GA = 1, G_GB = 2 };
 
 struct GemmArgs {
   int mode;              // G_SCORE / G_GA / G_GB
   int C;                 // chunks
-  int rowsA_per_chunk;   // M-dimension rows per chunk (Cs for SCORE/GA, Ns for GB)
-  int rowsB_per_chunk;   // N-dimension rows per chunk when B is K-major (Ns for SCORE)
-  int krows_per_chunk;   // K extent (D for SCORE, Ns for GA, Cs for GB)
-  int b_box_rows;        // rows of the TMA box of a K-major B operand (tile N of the tensor map)
-  int a_nblk, a_R;       // slab geometry of the A operand matrix: 32-column blocks per chunk, rows per chunk
+  int M, N, K;           // per-chunk extents (rows of A, rows of B, contraction)
+  int a_nblk, a_R;       // slab geometry of the A operand matrix: 32-column blocks per chunk, rows per block
   int b_nblk, b_R;       // same for the B operand matrix
   int model;
   float gamma, reg_coef;
@@ -52,253 +51,131 @@ struct GemmArgs {
   const float* a2;       // SCORE l2
   const float* b2;
   const float* colsum;   // GB l2
-  unsigned long long* dbg;   // optional per-CTA timestamps (KGE_B200_UMMA_TIMING=1): start, first full, mainloop end, end
 };
 
-// smem layout per stage: [A_hi | A_lo | B_hi | B_lo], each tile 1024-byte aligned
-template <bool A_MN, bool B_MN, int MODE>
+// smem layout per stage: [A_hi | A_lo | B_hi | B_lo], each tile 16 KB, 1024-byte aligned
+template <int MODE>
 __global__ void __launch_bounds__(kThreads, 1)
-k_umma_gemm(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-            const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, GemmArgs g) {
+k_wgmma_gemm(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+             const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, GemmArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages], tmem_full_bar;
-  __shared__ uint32_t tmem_base_slot;
-  __shared__ __align__(16) float b2s[256];     // |b_j|^2 of this tile's negatives (score epilogue)
+  __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages];
+  __shared__ __align__(16) float b2s[kTileN];     // |b_j|^2 of this tile's negatives (score epilogue)
 
-  const unsigned long long t_entry = gtime();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = blockIdx.z;
   const int m0 = blockIdx.y * kTileM;                 // row offset inside the chunk (M dimension)
-  const int n0 = blockIdx.x * 256;                    // column offset (N dimension)
-  const int Nleft = (MODE == G_SCORE ? g.Ns : g.D) - n0;
-  const int Nt = Nleft >= 256 ? 256 : ((Nleft + 15) & ~15);      // UMMA N (multiple of 16)
-  const int nblk = (Nt + 31) >> 5;                                // 32-wide MN blocks of B (MN-major)
-  const int K = g.krows_per_chunk;
-  const int num_kb = (K + kBlockK - 1) / kBlockK;
-
-  constexpr uint32_t kABytes = kTileM * 128;                      // one A tile (hi or lo): 128 rows x 128 B
-  const uint32_t bBytes = B_MN ? (uint32_t)nblk * 4096u : (uint32_t)g.b_box_rows * 128u;
-  const uint32_t bBytesAligned = (bBytes + 1023u) & ~1023u;
-  const uint32_t stageBytes = 2 * kABytes + 2 * bBytesAligned;
+  const int n0 = blockIdx.x * kTileN;                 // column offset (N dimension)
+  const int num_kb = (g.K + kBlockK - 1) / kBlockK;
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(&tmem_full_bar, 1);
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_slot)), "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_base_slot;
-  const int cta_lin = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-  if (g.dbg && threadIdx.x == 0) { g.dbg[cta_lin * 6 + 4] = t_entry; g.dbg[cta_lin * 6 + 0] = gtime(); }
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer (all lanes run the loop, one elected lane issues) =====================
-    {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (kb / kStages) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1);
-        uint8_t* st = smem + (size_t)s * stageBytes;
-        uint8_t* sAh = st; uint8_t* sAl = st + kABytes;
-        uint8_t* sBh = st + 2 * kABytes; uint8_t* sBl = sBh + bBytesAligned;
-        const int k0 = kb * kBlockK;
-        uint32_t tx = 2 * kABytes + 2 * bBytes;
-        if (elect_one()) {
-        mbar_expect_tx(&full_bar[s], tx);
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int s = kb % kStages;
+      const uint32_t ph = (kb / kStages) & 1;
+      mbar_wait(&empty_bar[s], ph ^ 1);
+      uint8_t* st = smem + (size_t)s * kStageBytes;
+      if (elect_one()) {
+        mbar_expect_tx(&full_bar[s], kStageBytes);
         // slab layout: row coordinate of (chunk c, 32-column block blk, row r) = (c * nblk + blk) * R + r; x = 0
-        if (!A_MN) {
-          // A K-major: column block = k-block kb, rows = M: one contiguous 16 KB box {32, 128 rows}
-          const int ya = (c * g.a_nblk + kb) * g.a_R + m0;
-          tma_load_2d(sAh, &tmAh, &full_bar[s], 0, ya);
-          tma_load_2d(sAl, &tmAl, &full_bar[s], 0, ya);
-        } else {
-          // A MN-major (stored [K rows][M cols]): column block = M block, rows = K: 4 contiguous boxes {32, 32 rows}
+        const int ya = (c * g.a_nblk + kb) * g.a_R + m0;
+        const int yb = (c * g.b_nblk + kb) * g.b_R + n0;
+        tma_load_2d(st, &tmAh, &full_bar[s], 0, ya);
+        tma_load_2d(st + kTileBytes, &tmAl, &full_bar[s], 0, ya);
+        tma_load_2d(st + 2 * kTileBytes, &tmBh, &full_bar[s], 0, yb);
+        tma_load_2d(st + 3 * kTileBytes, &tmBl, &full_bar[s], 0, yb);
+      }
+      __syncwarp();
+    }
+  } else if (warp < 8) {
+    // ===================== MMA + epilogue: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====================
+    const int wg = warp >> 2;
+    const bool l2 = g.model == KGE_TRANSE_L2;
+    if (MODE == G_SCORE && l2) {
+      // stage the tile's |b_j|^2 once (every row of the tile needs all of them) while the first loads are in flight
+      const int et = threadIdx.x;
+      if (et < kTileN) b2s[et] = (n0 + et < g.N) ? g.b2[(long long)c * g.Ns + n0 + et] : 0.f;
+      asm volatile("bar.sync 1, 256;" ::: "memory");   // the 8 consumer warps only
+    }
+    float acc[kTileN / 2];
 #pragma unroll
-          for (int b = 0; b < kTileM / 32; ++b) {
-            const int ya = (c * g.a_nblk + (m0 >> 5) + b) * g.a_R + k0;
-            tma_load_2d(sAh + b * 4096, &tmAh, &full_bar[s], 0, ya);
-            tma_load_2d(sAl + b * 4096, &tmAl, &full_bar[s], 0, ya);
-          }
-        }
-        if (!B_MN) {
-          const int yb = (c * g.b_nblk + kb) * g.b_R + n0;
-          tma_load_2d(sBh, &tmBh, &full_bar[s], 0, yb);
-          tma_load_2d(sBl, &tmBl, &full_bar[s], 0, yb);
-        } else {
-          for (int b = 0; b < nblk; ++b) {
-            const int yb = (c * g.b_nblk + (n0 >> 5) + b) * g.b_R + k0;
-            tma_load_2d(sBh + b * 4096, &tmBh, &full_bar[s], 0, yb);
-            tma_load_2d(sBl + b * 4096, &tmBl, &full_bar[s], 0, yb);
-          }
-        }
-        }   // elect_one
-        __syncwarp();
+    for (int i = 0; i < kTileN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int s = kb % kStages;
+      mbar_wait(&full_bar[s], (kb / kStages) & 1);
+      const uint32_t st = smem_u32(smem + (size_t)s * kStageBytes);
+      const uint64_t dAh = make_desc(st + wg * 8192u), dAl = make_desc(st + kTileBytes + wg * 8192u);
+      const uint64_t dBh = make_desc(st + 2 * kTileBytes), dBl = make_desc(st + 3 * kTileBytes);
+      const int kleft = g.K - kb * kBlockK;
+      const int ksteps = kleft >= kBlockK ? kBlockK / kMmaK : kleft / kMmaK;   // K % 8 == 0 guaranteed
+      wgmma_fence();
+      for (int ks = 0; ks < ksteps; ++ks) {
+        const uint64_t o = (uint64_t)(ks * 2);     // +32 bytes per k-step inside the 128-byte swizzle span
+        wgmma_ss<kTileN>(acc, dAh + o, dBh + o, 1u);
+        wgmma_ss<kTileN>(acc, dAh + o, dBl + o, 1u);
+        wgmma_ss<kTileN>(acc, dAl + o, dBh + o, 1u);
+      }
+      wgmma_commit();
+      if (kb > 0) {
+        wgmma_wait<1>();                             // the previous k-block's MMAs have retired: its stage is free
+        if (lane == 0) mbar_arrive(&empty_bar[(kb - 1) % kStages]);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    {
-      const uint32_t idesc = make_idesc(kTileM, Nt, A_MN, B_MN);
-      uint32_t accumulate = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (kb / kStages) & 1;
-        mbar_wait(&full_bar[s], ph);
-        if (g.dbg && kb == 0 && lane == 0) g.dbg[cta_lin * 6 + 1] = gtime();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t st = smem_u32(smem + (size_t)s * stageBytes);
-        const uint32_t sAh = st, sAl = st + kABytes, sBh = st + 2 * kABytes, sBl = sBh + bBytesAligned;
-        const int kleft = K - kb * kBlockK;
-        const int ksteps = kleft >= kBlockK ? kBlockK / kUmmaK : kleft / kUmmaK;   // K % 8 == 0 guaranteed
-        if (elect_one()) {
-        for (int ks = 0; ks < ksteps; ++ks) {
-          // K-major: +32 bytes per k-step inside the 128-byte swizzle span; SBO = 1024 (8-row groups)
-          // MN-major (128B swizzle, 32B atoms): k-atoms of 4 rows (512 B, SBO), one k-step = 2 atoms = 1024 B;
-          // LBO = 4096 between 32-wide MN blocks
-          const uint32_t aoff = A_MN ? ks * 1024u : ks * 32u;
-          const uint32_t boff = B_MN ? ks * 1024u : ks * 32u;
-          const uint64_t dAh = A_MN ? make_desc(sAh + aoff, 4096, 512, 1) : make_desc(sAh + aoff, 16, 1024);
-          const uint64_t dAl = A_MN ? make_desc(sAl + aoff, 4096, 512, 1) : make_desc(sAl + aoff, 16, 1024);
-          const uint64_t dBh = B_MN ? make_desc(sBh + boff, 4096, 512, 1) : make_desc(sBh + boff, 16, 1024);
-          const uint64_t dBl = B_MN ? make_desc(sBl + boff, 4096, 512, 1) : make_desc(sBl + boff, 16, 1024);
-          umma_tf32(tmem_base, dAh, dBh, idesc, (accumulate | (uint32_t)ks) ? 1u : 0u);
-          umma_tf32(tmem_base, dAh, dBl, idesc, 1u);
-          umma_tf32(tmem_base, dAl, dBh, idesc, 1u);
-        }
-        umma_commit(&empty_bar[s]);          // frees the smem stage when these MMAs retire
-        if (kb == num_kb - 1) umma_commit(&tmem_full_bar);           // accumulator complete
-        }   // elect_one
-        accumulate = 1u;
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===================== epilogue: warps 2..9, TMEM lane quarter = warp % 4 =====================
-    if (MODE == G_SCORE && g.model == KGE_TRANSE_L2) {
-      // stage the tile's |b_j|^2 once (every row of the tile needs all of them) while the mainloop runs
-      const int et = threadIdx.x - 64;                 // 0..255
-      if (et < 256) b2s[et] = (n0 + et < g.Ns) ? g.b2[(long long)c * g.Ns + n0 + et] : 0.f;
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // the 8 epilogue warps only
-    }
-    mbar_wait(&tmem_full_bar, 0);
-    if (g.dbg && threadIdx.x == 64) g.dbg[cta_lin * 6 + 2] = gtime();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int q = warp & 3;
-    // two warps share a TMEM lane quarter and split the tile's columns
-    const int ehalf = (warp - 2) >> 2;
-    const int Nt_half = ((Nt >> 1) + 15) & ~15;
-    const int col_begin = ehalf ? Nt_half : 0;
-    const int col_end = ehalf ? Nt : Nt_half;
-    const int row_in_tile = q * 32 + lane;                 // accumulator row (M index) owned by this thread
-    const int m = m0 + row_in_tile;
-    const int Mrows = g.rowsA_per_chunk;
-    const bool row_ok = m < Mrows;
-    const uint32_t taddr_row = tmem_base + ((uint32_t)(q * 32) << 16);
-    // Nt is a multiple of 16; Ns, D are multiples of 8: every 8-column group is entirely valid or entirely padding
-    if (MODE == G_SCORE) {
-      const long long gi = (long long)c * g.Cs + m;
-      const bool l2 = g.model == KGE_TRANSE_L2;
-      const float a2v = (row_ok && l2) ? g.a2[gi] : 0.f;
-      for (int col = col_begin; col < col_end; col += 16) {
-        float v[16];
-        tmem_ld16(taddr_row + col, v);
-        if (!row_ok) continue;
+    wgmma_wait<0>();
+    reg_fence(acc);
+
+    // epilogue from the accumulator fragment: rows r0, r0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
+    const int q = lane & 3;
 #pragma unroll
-        for (int h8 = 0; h8 < 2; ++h8) {
-          const int j = n0 + col + h8 * 8;
-          if (j >= g.Ns) continue;
-          float sc[8];
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      if (m >= g.M) continue;
+      if (MODE == G_SCORE) {
+        const long long gi = (long long)c * g.Cs + m;
+        const float a2v = l2 ? g.a2[gi] : 0.f;
+#pragma unroll
+        for (int j = 0; j < kTileN / 8; ++j) {
+          const int col = 8 * j + 2 * q, n = n0 + col;
+          if (n >= g.N) continue;
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
           if (l2) {
             // batched_l2_dist (score_fun.py:26-34): (|b|^2 - 2 a.b) + |a|^2, clamp, sqrt
-            float4 bq0 = *reinterpret_cast<const float4*>(&b2s[j - n0]), bq1 = *reinterpret_cast<const float4*>(&b2s[j - n0 + 4]);
-            const float bb[8] = {bq0.x, bq0.y, bq0.z, bq0.w, bq1.x, bq1.y, bq1.z, bq1.w};
-            float d[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              float sq = fmaf(-2.f, v[h8 * 8 + e], bb[e]) + a2v;
-              d[e] = sqrtf(fmaxf(sq, 1e-30f));
-              sc[e] = g.gamma - d[e];
-            }
-            st4(g.out2 + gi * g.Ns + j, make_float4(d[0], d[1], d[2], d[3]));
-            st4(g.out2 + gi * g.Ns + j + 4, make_float4(d[4], d[5], d[6], d[7]));
-          } else {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) sc[e] = v[h8 * 8 + e];
+            const float d0 = sqrtf(fmaxf(fmaf(-2.f, v0, b2s[col]) + a2v, 1e-30f));
+            const float d1 = sqrtf(fmaxf(fmaf(-2.f, v1, b2s[col + 1]) + a2v, 1e-30f));
+            *reinterpret_cast<float2*>(g.out2 + gi * g.Ns + n) = make_float2(d0, d1);
+            v0 = g.gamma - d0; v1 = g.gamma - d1;
           }
-          st4(g.out + gi * g.Ns + j, make_float4(sc[0], sc[1], sc[2], sc[3]));
-          st4(g.out + gi * g.Ns + j + 4, make_float4(sc[4], sc[5], sc[6], sc[7]));
+          *reinterpret_cast<float2*>(g.out + gi * g.Ns + n) = make_float2(v0, v1);
         }
-      }
-    } else if (MODE == G_GA) {
-      float* row = g.out + ((long long)c * g.Cs + m) * g.D;
-      for (int col = col_begin; col < col_end; col += 16) {
-        float v[16];
-        tmem_ld16(taddr_row + col, v);
-        if (!row_ok) continue;
+      } else if (MODE == G_GA) {
+        float* row = g.out + ((long long)c * g.Cs + m) * g.D;
 #pragma unroll
-        for (int h8 = 0; h8 < 2; ++h8) {
-          const int k = n0 + col + h8 * 8;
-          if (k >= g.D) continue;
-          st4(row + k, make_float4(v[h8 * 8 + 0], v[h8 * 8 + 1], v[h8 * 8 + 2], v[h8 * 8 + 3]));
-          st4(row + k + 4, make_float4(v[h8 * 8 + 4], v[h8 * 8 + 5], v[h8 * 8 + 6], v[h8 * 8 + 7]));
+        for (int j = 0; j < kTileN / 8; ++j) {
+          const int k = n0 + 8 * j + 2 * q;
+          if (k < g.N) *reinterpret_cast<float2*>(row + k) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
-      }
-    } else {  // G_GB: gradient of the negative rows, written over the gathered rows
-      float* row = g.out + ((long long)c * g.Ns + m) * g.D;
-      const bool l2 = g.model == KGE_TRANSE_L2;
-      const float cs = (row_ok && l2) ? g.colsum[(long long)c * g.Ns + m] : 0.f;
-      // the row's own values b (for -colsum*b and the regulariser) are prefetched one 16-column chunk ahead so
-      // that their global-memory latency overlaps the TMEM load + math + stores of the current chunk
-      float4 bcur[4], bnxt[4];
-      auto load_b = [&](int col, float4* dst) {
+      } else {  // G_GB: gradient of the negative rows, written over the gathered rows
+        float* row = g.out + ((long long)c * g.Ns + m) * g.D;
+        const float cs = l2 ? g.colsum[(long long)c * g.Ns + m] : 0.f;
 #pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {
-          const int k = n0 + col + q4 * 4;
-          dst[q4] = (row_ok && col < col_end && k < g.D) ? ld4(row + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int j = 0; j < kTileN / 8; ++j) {
+          const int k = n0 + 8 * j + 2 * q;
+          if (k >= g.N) continue;
+          const float2 b = *reinterpret_cast<const float2*>(row + k);
+          float g0 = acc[4 * j + 2 * h], g1 = acc[4 * j + 2 * h + 1];
+          if (l2) { g0 = fmaf(-cs, b.x, g0); g1 = fmaf(-cs, b.y, g1); }     // sum_i V_ij a_i - (sum_i V_ij) b_j
+          *reinterpret_cast<float2*>(row + k) = make_float2(g0 + reg_grad(b.x, g.reg_norm, g.reg_coef),
+                                                            g1 + reg_grad(b.y, g.reg_norm, g.reg_coef));
         }
-      };
-      load_b(col_begin, bcur);
-      for (int col = col_begin; col < col_end; col += 16) {
-        load_b(col + 16, bnxt);
-        float v[16];
-        tmem_ld16(taddr_row + col, v);
-        if (row_ok) {
-#pragma unroll
-          for (int h8 = 0; h8 < 2; ++h8) {
-            const int k = n0 + col + h8 * 8;
-            if (k >= g.D) continue;
-            const float4 b0 = bcur[h8 * 2], b1 = bcur[h8 * 2 + 1];
-            const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-            float o[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              float gv = v[h8 * 8 + e];
-              if (l2) gv = fmaf(-cs, bb[e], gv);                 // sum_i V_ij a_i - (sum_i V_ij) b_j
-              o[e] = gv + reg_grad(bb[e], g.reg_norm, g.reg_coef);
-            }
-            st4(row + k, make_float4(o[0], o[1], o[2], o[3]));
-            st4(row + k + 4, make_float4(o[4], o[5], o[6], o[7]));
-          }
-        }
-#pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) bcur[q4] = bnxt[q4];
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  if (g.dbg && threadIdx.x == 0) g.dbg[cta_lin * 6 + 3] = gtime();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
-    if (g.dbg && lane == 0) g.dbg[cta_lin * 6 + 5] = gtime();
   }
 }
 
@@ -319,9 +196,9 @@ encode_fn_t get_encode() {
   return fn;
 }
 
-// cuTensorMapEncodeTiled costs ~0.1 ms per call on this driver; the workspace matrices keep their
+// cuTensorMapEncodeTiled is a host-side driver call per map; the workspace matrices keep their
 // addresses between steps, so the encoded maps are cached (per host thread).
-struct MapKey { const void* base; long long rows, cols; int box_rows; bool mn; int dev; };
+struct MapKey { const void* base; long long rows, cols; int box_rows; int dev; };
 struct MapCache {
   static constexpr int kN = 64;
   MapKey keys[kN];
@@ -331,30 +208,29 @@ struct MapCache {
 thread_local MapCache g_maps;
 
 bool make_map_uncached(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err,
-                       size_t errlen, bool mn_major);
+                       size_t errlen);
 
-bool make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen,
-              bool mn_major = false) {
+bool make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen) {
   MapCache& mc = g_maps;
   int dev = 0;
   cudaGetDevice(&dev);
   for (int i = 0; i < mc.n; ++i) {
     const MapKey& k = mc.keys[i];
-    if (k.base == base && k.rows == rows && k.cols == cols && k.box_rows == box_rows && k.mn == mn_major && k.dev == dev) {
+    if (k.base == base && k.rows == rows && k.cols == cols && k.box_rows == box_rows && k.dev == dev) {
       *m = mc.maps[i];
       return true;
     }
   }
-  if (!make_map_uncached(m, base, rows, cols, box_rows, err, errlen, mn_major)) return false;
+  if (!make_map_uncached(m, base, rows, cols, box_rows, err, errlen)) return false;
   int slot = mc.n < MapCache::kN ? mc.n++ : (mc.next++ % MapCache::kN);
-  mc.keys[slot] = MapKey{base, rows, cols, box_rows, mn_major, dev};
+  mc.keys[slot] = MapKey{base, rows, cols, box_rows, dev};
   mc.maps[slot] = *m;
   return true;
 }
 
 // 2-D fp32 row-major matrix [rows, cols], box {32 cols, box_rows}, 128-byte swizzle, zero OOB fill
 bool make_map_uncached(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err,
-                       size_t errlen, bool mn_major) {
+                       size_t errlen) {
   encode_fn_t enc = get_encode();
   if (!enc) { snprintf(err, errlen, "cuTensorMapEncodeTiled not available"); return false; }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
@@ -362,70 +238,38 @@ bool make_map_uncached(CUtensorMap* m, const float* base, long long rows, long l
   cuuint32_t box[2] = {32u, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1u, 1u};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { snprintf(err, errlen, "cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld box_rows=%d", (int)r, rows, cols, box_rows); return false; }
   return true;
 }
 
-size_t smem_bytes_for(int Nt, bool b_mn) {
-  const int nblk = (Nt + 31) >> 5;
-  size_t b = b_mn ? (size_t)nblk * 4096 : (size_t)Nt * 128;
-  b = (b + 1023) & ~(size_t)1023;
-  return (size_t)kStages * (2 * kTileM * 128 + 2 * b) + 1024;
-}
-
-template <bool A_MN, bool B_MN, int MODE>
+template <int MODE>
 int launch_gemm(const LaunchCtx& c, const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
-                const CUtensorMap& bl, const GemmArgs& g, int ntiles_n, int Nt_max, char* err, size_t errlen) {
-  size_t smem = smem_bytes_for(Nt_max, B_MN);
+                const CUtensorMap& bl, const GemmArgs& g, char* err, size_t errlen) {
+  const size_t smem = (size_t)kStages * kStageBytes + 1024;
   static bool attr_set[64] = {};          // the opt-in shared-memory size is a per-device function attribute
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_umma_gemm<A_MN, B_MN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_wgmma_gemm<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { snprintf(err, errlen, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return KGE_ERR_CUDA; }
     attr_set[dev] = true;
   }
-  dim3 grid(ntiles_n, (g.rowsA_per_chunk + kTileM - 1) / kTileM, g.C);
-  const char* nm = MODE == G_SCORE ? "k_umma_gemm<score S=A.Bn^T>"
-                                   : (MODE == G_GA ? "k_umma_gemm<grad_a GA=V.Bn>" : "k_umma_gemm<grad_b GB=V^T.A>");
-  static const bool timing = getenv("KGE_B200_UMMA_TIMING") != nullptr;
-  GemmArgs ga = g;
-  unsigned long long* dbg = nullptr;
-  const size_t nct = (size_t)grid.x * grid.y * grid.z;
-  if (timing) { cudaMalloc(&dbg, nct * 6 * sizeof(unsigned long long)); ga.dbg = dbg; }
-  KGE_LAUNCH_NAMED(c, nm, (k_umma_gemm<A_MN, B_MN, MODE>), grid, kThreads, smem, ah, al, bh, bl, ga);
-  if (timing) {
-    cudaStreamSynchronize(c.stream);
-    unsigned long long* hbuf = (unsigned long long*)malloc(nct * 6 * sizeof(unsigned long long));
-    cudaMemcpy(hbuf, dbg, nct * 6 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-    double t1 = 0, t2 = 0, t3 = 0, ta = 0, td = 0; unsigned long long mn = ~0ull, mx = 0, mne = ~0ull, mxd = 0;
-    for (size_t i = 0; i < nct; ++i) {
-      const unsigned long long* r = hbuf + i * 6;
-      t1 += (double)(r[1] - r[0]); t2 += (double)(r[2] - r[0]); t3 += (double)(r[3] - r[0]);
-      ta += (double)(r[0] - r[4]); td += (double)(r[5] - r[3]);
-      if (r[0] < mn) mn = r[0];
-      if (r[3] > mx) mx = r[3];
-      if (r[4] < mne) mne = r[4];
-      if (r[5] > mxd) mxd = r[5];
-    }
-    fprintf(stderr, "[umma timing] %s ctas=%zu alloc=%.2fus first_full=%.2fus mainloop_end=%.2fus cta_end=%.2fus dealloc=%.2fus "
-            "span(after alloc..before dealloc)=%.2fus span(entry..after dealloc)=%.2fus\n", nm, nct, ta / nct / 1e3, t1 / nct / 1e3,
-            t2 / nct / 1e3, t3 / nct / 1e3, td / nct / 1e3, (double)(mx - mn) / 1e3, (double)(mxd - mne) / 1e3);
-    free(hbuf); cudaFree(dbg);
-  }
+  dim3 grid((g.N + kTileN - 1) / kTileN, (g.M + kTileM - 1) / kTileM, g.C);
+  const char* nm = MODE == G_SCORE ? "k_wgmma_gemm<score S=A.Bn^T>"
+                                   : (MODE == G_GA ? "k_wgmma_gemm<grad_a GA=V.Bn>" : "k_wgmma_gemm<grad_b GB=V^T.A>");
+  KGE_LAUNCH_NAMED(c, nm, (k_wgmma_gemm<MODE>), grid, kThreads, smem, ah, al, bh, bl, g);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { snprintf(err, errlen, "umma launch: %s", cudaGetErrorString(e)); return KGE_ERR_CUDA; }
+  if (e != cudaSuccess) { snprintf(err, errlen, "wgmma gemm launch: %s", cudaGetErrorString(e)); return KGE_ERR_CUDA; }
   return KGE_OK;
 }
 
 }  // namespace
 
-bool tc_make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen,
-                 bool mn_major) {
-  return make_map(m, base, rows, cols, box_rows, err, errlen, mn_major);
+bool tc_make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen) {
+  return make_map(m, base, rows, cols, box_rows, err, errlen);
 }
 
 bool umma_supported(const StepParams& p) {
@@ -433,50 +277,53 @@ bool umma_supported(const StepParams& p) {
   return model_ok && (p.D % 8 == 0) && (p.Cs % 8 == 0) && (p.Ns % 8 == 0) && p.D >= 32 && p.Cs >= 8 && p.Ns >= 8;
 }
 
+namespace {
+GemmArgs base_args(const StepParams& p) {
+  GemmArgs g{};
+  g.C = p.C; g.model = p.model; g.gamma = p.gamma; g.reg_coef = p.reg_coef; g.reg_norm = p.reg_norm;
+  g.Cs = p.Cs; g.Ns = p.Ns; g.D = p.D;
+  return g;
+}
+}  // namespace
+
 // S = A . Bn^T  (+ TransE_l2 distance epilogue)
 int umma_score(const LaunchCtx& c, const StepParams& p, const StepWs& w, char* err, size_t errlen) {
   // operands arrive already split: k_prep writes A / Bn as TF32 hi/lo, k_loss writes V hi/lo
-  const int Nt_max = p.Ns >= 256 ? 256 : ((p.Ns + 15) & ~15);
   CUtensorMap ah, al, bh, bl;
   const long long rowsA = p.B * (long long)slab_blocks(p.D), rowsB = p.Nn * (long long)slab_blocks(p.D);
   if (!make_map(&ah, w.Ahi, rowsA, 32, kTileM, err, errlen) || !make_map(&al, w.Alo, rowsA, 32, kTileM, err, errlen) ||
-      !make_map(&bh, w.Bhi, rowsB, 32, Nt_max, err, errlen) || !make_map(&bl, w.Blo, rowsB, 32, Nt_max, err, errlen))
+      !make_map(&bh, w.Bhi, rowsB, 32, kTileN, err, errlen) || !make_map(&bl, w.Blo, rowsB, 32, kTileN, err, errlen))
     return KGE_ERR_CUDA;
-  GemmArgs g{};
-  g.mode = G_SCORE; g.C = p.C; g.rowsA_per_chunk = p.Cs; g.rowsB_per_chunk = p.Ns; g.krows_per_chunk = p.D;
-  g.b_box_rows = Nt_max;
+  GemmArgs g = base_args(p);
+  g.mode = G_SCORE; g.M = p.Cs; g.N = p.Ns; g.K = p.D;
   g.a_nblk = slab_blocks(p.D); g.a_R = p.Cs; g.b_nblk = slab_blocks(p.D); g.b_R = p.Ns;
-  g.model = p.model; g.gamma = p.gamma; g.reg_coef = p.reg_coef; g.reg_norm = p.reg_norm;
-  g.Cs = p.Cs; g.Ns = p.Ns; g.D = p.D;
-  g.out = w.S; g.out2 = w.V; g.a2 = w.a2; g.b2 = w.b2; g.colsum = nullptr;
-  return launch_gemm<false, false, G_SCORE>(c, ah, al, bh, bl, g, (p.Ns + 255) / 256, Nt_max, err, errlen);
+  g.out = w.S; g.out2 = w.V; g.a2 = w.a2; g.b2 = w.b2;
+  return launch_gemm<G_SCORE>(c, ah, al, bh, bl, g, err, errlen);
 }
 
 // side_b == false: GA = V . Bn ; side_b == true: G_neg = V^T . A (+ epilogue), in place over Bn
 int umma_grad(const LaunchCtx& c, const StepParams& p, const StepWs& w, bool side_b, char* err, size_t errlen) {
-  const int Nt_max = p.D >= 256 ? 256 : ((p.D + 15) & ~15);
   CUtensorMap ah, al, bh, bl;
-  GemmArgs g{};
-  g.C = p.C; g.model = p.model; g.gamma = p.gamma; g.reg_coef = p.reg_coef; g.reg_norm = p.reg_norm;
-  g.Cs = p.Cs; g.Ns = p.Ns; g.D = p.D; g.colsum = w.colsum;
+  GemmArgs g = base_args(p);
+  g.colsum = w.colsum;
   if (!side_b) {
-    // A operand: V [B, Ns] K-major (K = j); B operand: Bn hi/lo [Nn, D] MN-major (rows = K = j, cols = N = k)
-    const long long rowsV = p.B * (long long)slab_blocks(p.Ns), rowsB = p.Nn * (long long)slab_blocks(p.D);
+    // A operand: V slabs [C][Ns/32][Cs][32]; B operand: Bn^T slabs [C][Ns/32][D][32]; K = j
+    const long long rowsV = p.B * (long long)slab_blocks(p.Ns), rowsB = (long long)p.C * slab_blocks(p.Ns) * p.D;
     if (!make_map(&ah, w.Vhi, rowsV, 32, kTileM, err, errlen) || !make_map(&al, w.Vlo, rowsV, 32, kTileM, err, errlen) ||
-        !make_map(&bh, w.Bhi, rowsB, 32, 32, err, errlen, true) || !make_map(&bl, w.Blo, rowsB, 32, 32, err, errlen, true))
+        !make_map(&bh, w.BhiT, rowsB, 32, kTileN, err, errlen) || !make_map(&bl, w.BloT, rowsB, 32, kTileN, err, errlen))
       return KGE_ERR_CUDA;
-    g.a_nblk = slab_blocks(p.Ns); g.a_R = p.Cs; g.b_nblk = slab_blocks(p.D); g.b_R = p.Ns;
-    g.mode = G_GA; g.rowsA_per_chunk = p.Cs; g.rowsB_per_chunk = 0; g.krows_per_chunk = p.Ns; g.out = w.GA;
-    return launch_gemm<false, true, G_GA>(c, ah, al, bh, bl, g, (p.D + 255) / 256, Nt_max, err, errlen);
+    g.a_nblk = slab_blocks(p.Ns); g.a_R = p.Cs; g.b_nblk = slab_blocks(p.Ns); g.b_R = p.D;
+    g.mode = G_GA; g.M = p.Cs; g.N = p.D; g.K = p.Ns; g.out = w.GA;
+    return launch_gemm<G_GA>(c, ah, al, bh, bl, g, err, errlen);
   }
-  // A operand: V^T: stored V [B, Ns] = [rows = K = i][cols = M = j] MN-major; B operand: A hi/lo [B, D] MN-major
-  const long long rowsV = p.B * (long long)slab_blocks(p.Ns), rowsA = p.B * (long long)slab_blocks(p.D);
-  if (!make_map(&ah, w.Vhi, rowsV, 32, 32, err, errlen, true) || !make_map(&al, w.Vlo, rowsV, 32, 32, err, errlen, true) ||
-      !make_map(&bh, w.Ahi, rowsA, 32, 32, err, errlen, true) || !make_map(&bl, w.Alo, rowsA, 32, 32, err, errlen, true))
+  // A operand: V^T slabs [C][Cs/32][Ns][32]; B operand: A^T slabs [C][Cs/32][D][32]; K = i
+  const long long rowsV = (long long)p.C * slab_blocks(p.Cs) * p.Ns, rowsA = (long long)p.C * slab_blocks(p.Cs) * p.D;
+  if (!make_map(&ah, w.VhiT, rowsV, 32, kTileM, err, errlen) || !make_map(&al, w.VloT, rowsV, 32, kTileM, err, errlen) ||
+      !make_map(&bh, w.AhiT, rowsA, 32, kTileN, err, errlen) || !make_map(&bl, w.AloT, rowsA, 32, kTileN, err, errlen))
     return KGE_ERR_CUDA;
-  g.a_nblk = slab_blocks(p.Ns); g.a_R = p.Cs; g.b_nblk = slab_blocks(p.D); g.b_R = p.Cs;
-  g.mode = G_GB; g.rowsA_per_chunk = p.Ns; g.rowsB_per_chunk = 0; g.krows_per_chunk = p.Cs; g.out = w.Bn;
-  return launch_gemm<true, true, G_GB>(c, ah, al, bh, bl, g, (p.D + 255) / 256, Nt_max, err, errlen);
+  g.a_nblk = slab_blocks(p.Cs); g.a_R = p.Ns; g.b_nblk = slab_blocks(p.Cs); g.b_R = p.D;
+  g.mode = G_GB; g.M = p.Ns; g.N = p.D; g.K = p.Cs; g.out = w.Bn;
+  return launch_gemm<G_GB>(c, ah, al, bh, bl, g, err, errlen);
 }
 
 }  // namespace kge

@@ -1,6 +1,6 @@
 """ctypes binding of libkge_b200.so (include/kge_b200.h).
 
-There is NO fallback: if the shared library is missing, cannot be loaded, or no sm_100 GPU is
+There is NO fallback: if the shared library is missing, cannot be loaded, or no sm_90 GPU is
 visible, every entry point raises.  The structures below mirror the C header field by field.
 """
 import ctypes as C
@@ -132,7 +132,7 @@ class Handle:
     def __init__(self, device=0):
         lib = load_library()
         if not torch.cuda.is_available():
-            raise KgeError("no CUDA device: libkge_b200 is a B200 (sm_100a) library and has no CPU path")
+            raise KgeError("no CUDA device: libkge_b200 is an H100 (sm_90a) library and has no CPU path")
         self.device = torch.device("cuda", device if isinstance(device, int) else device.index)
         self._h = C.c_void_p()
         check(lib.kge_create(self.device.index, C.byref(self._h)))
@@ -163,7 +163,7 @@ class Handle:
         check(self.lib.kge_set_engine(self._h, int(engine)))
 
     def set_fused(self, mode):
-        """-1 / 1: fused tcgen05 contraction kernel when the shape allows (default); 0: separate GEMM + loss kernels."""
+        """-1 / 1: fused wgmma contraction kernel when the shape allows (default); 0: separate GEMM + loss kernels."""
         check(self.lib.kge_set_fused(self._h, int(mode)))
 
     def set_dump(self, tensor):

@@ -52,7 +52,7 @@ class KEModel(object):
                                       "table + NCCL all-reduce of dglke_b200.dist")
         device = get_device(args)
         if device.type != "cuda":
-            raise _lib.KgeError("KEModel needs --gpu >= 0: the B200 library has no CPU path")
+            raise _lib.KgeError("KEModel needs --gpu >= 0: the library has no CPU path")
         self.device = device
         self.loss_gen = LossGenerator(args, getattr(args, "loss_genre", "Logsigmoid"),
                                       getattr(args, "neg_adversarial_sampling", False),
@@ -209,10 +209,10 @@ class KEModel(object):
         self.entity_emb.finish_async_update()
 
     def prepare_relation(self, device=None):
-        raise NotImplementedError("relation partitioning is not used by the B200 multi-GPU path")
+        raise NotImplementedError("relation partitioning is not used by this multi-GPU path")
 
     def writeback_relation(self, rank=0, rel_parts=None):
-        raise NotImplementedError("relation partitioning is not used by the B200 multi-GPU path")
+        raise NotImplementedError("relation partitioning is not used by this multi-GPU path")
 
     def load_relation(self, device=None):
-        raise NotImplementedError("relation partitioning is not used by the B200 multi-GPU path")
+        raise NotImplementedError("relation partitioning is not used by this multi-GPU path")

@@ -2,7 +2,7 @@
 
 All four criteria of the reference (Hinge, Logistic, Logsigmoid, BCE: loss.py:10-38), the self-adversarial negative
 weighting, edge-importance weights and the pairwise form (loss.py:76-80) run in the library (k_loss; the Logsigmoid family
-without -pw also inside the fused tcgen05 kernel).  Logistic and BCE are the Logsigmoid criterion written differently and
+without -pw also inside the fused wgmma kernel).  Logistic and BCE are the Logsigmoid criterion written differently and
 share its kernels; the same argument errors as the reference's are raised (loss.py:58-62, base_loss.py:83-84)."""
 import torch as th
 

@@ -58,7 +58,7 @@ class ExternalEmbedding:
             # --mix_cpu_gpu's host-resident table is replaced by HBM-resident (optionally sharded) tables
             device = th.device("cuda", th.cuda.current_device()) if th.cuda.is_available() else device
         if device.type != "cuda":
-            raise E._lib.KgeError("ExternalEmbedding needs a CUDA device: the B200 library has no CPU path")
+            raise E._lib.KgeError("ExternalEmbedding needs a CUDA device: the library has no CPU path")
         self.gpu = getattr(args, "gpu", [device.index])
         self.args = args
         self.num, self.dim = num, dim

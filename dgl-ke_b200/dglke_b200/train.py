@@ -148,7 +148,7 @@ def test(args, model, batches, rank=0, mode="Test"):
 def main(argv=None):
     args = ArgParser().parse_args(argv)
     if args.gpu[0] < 0:
-        raise SystemExit("dglke_b200 needs --gpu: the hot path is a B200 CUDA library without a CPU fallback")
+        raise SystemExit("dglke_b200 needs --gpu: the hot path is an H100 CUDA library without a CPU fallback")
     prepare_save_path(args)
     args.eval_filter = not args.no_eval_filter
     args.strict_rel_part = args.soft_rel_part = False

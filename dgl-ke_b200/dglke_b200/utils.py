@@ -90,4 +90,4 @@ class ArgParser(CommonArgParser):
         A("--rel_part", action="store_true", help="relation partitioning (not needed: relations are replicated)")
         A("--async_update", action="store_true", help="asynchronous entity update (always stream-async here)")
         A("--has_edge_importance", action="store_true", help="edges carry an importance weight")
-        A("--host_sampler", action="store_true", help="(B200 only) sample on the host with numpy instead of on the GPU")
+        A("--host_sampler", action="store_true", help="(this package only) sample on the host with numpy instead of on the GPU")

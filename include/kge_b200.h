@@ -1,5 +1,5 @@
 /*
- * kge_b200.h -- C ABI of libkge_b200.so: the B200-native (sm_100a) replacement for the
+ * kge_b200.h -- C ABI of libkge_b200.so: the H100-native (sm_90a) replacement for the
  * per-step hot path of awslabs/dgl-ke's `dglke_train`:
  *
  *   ExternalEmbedding gather  ->  score_func over 1 positive + chunk-shared negatives
@@ -7,7 +7,7 @@
  *
  * The reference has no native layer (it is pure Python on top of PyTorch ATen); each entry
  * point below therefore cites the *Python* function it replaces, with file:line relative to
- * /root/reference/python/dglke.  The host side (dgl-ke_b200/dglke_b200) binds this header with
+ * python/dglke of awslabs/dgl-ke.  The host side (dgl-ke_b200/dglke_b200) binds this header with
  * ctypes and mirrors the reference's KEModel / score_func / ExternalEmbedding surface.
  *
  * Conventions
@@ -46,7 +46,7 @@ typedef enum {
   KGE_ERR_UNSUPPORTED = -2,   /* model/dim combination this build does not implement              */
   KGE_ERR_CUDA = -3,          /* a CUDA runtime call failed; see kge_last_error()                  */
   KGE_ERR_NOMEM = -4,         /* workspace allocation failed                                       */
-  KGE_ERR_NO_DEVICE = -5      /* no usable sm_100 device                                           */
+  KGE_ERR_NO_DEVICE = -5      /* no usable sm_90 device                                            */
 } kge_status;
 
 /* models/general_models.py:238-258 (model_name -> score_func) */
@@ -142,7 +142,7 @@ KGE_API int kge_abi_version(void);
 KGE_API const char* kge_last_error(void);
 
 /* Creates the per-device context (workspace, pinned staging, SM count).  `device` is a CUDA
- * ordinal.  Fails with KGE_ERR_NO_DEVICE when no sm_100 GPU is present -- there is no CPU path. */
+ * ordinal.  Fails with KGE_ERR_NO_DEVICE when no sm_90 GPU is present -- there is no CPU path. */
 KGE_API int kge_create(int device, kge_handle_t* out);
 KGE_API int kge_destroy(kge_handle_t h);
 
@@ -259,12 +259,12 @@ KGE_API int64_t kge_launch_count(kge_handle_t h);
  * durations in milliseconds, returns the record count and starts a new record set. */
 KGE_API int kge_profile_enable(kge_handle_t h, int on);
 KGE_API int kge_profile_read(kge_handle_t h, char* names, int names_len, float* ms, int max_records);
-/* Selects the contraction engine: 0 = fp32 CUDA-core tiles, 1 = tcgen05 3xTF32 tensor-core tiles
+/* Selects the contraction engine: 0 = fp32 CUDA-core tiles, 1 = wgmma 3xTF32 tensor-core tiles
  * (bilinear models), -1 = library default. */
 KGE_API int kge_set_engine(kge_handle_t h, int engine);
 
-/* Selects the contraction schedule of the bilinear / L2 models: -1 (default) or 1 = the fused tcgen05 kernel
- * (score -> loss -> coefficients in TMEM -> gradient GEMM, kge_fused.cu) whenever the chunk shape fits its TMEM budget
+/* Selects the contraction schedule of the bilinear / L2 models: -1 (default) or 1 = the fused wgmma kernel
+ * (score -> loss -> coefficients in registers -> gradient GEMM, kge_fused.cu) whenever the chunk shape fits its register budget
  * (chunk_size, neg_sample_size <= 240), 0 = separate GEMM / loss kernels. */
 KGE_API int kge_set_fused(kge_handle_t h, int mode);
 /* Test hook: when non-null, the fused kernel also writes its backward coefficients dL/dneg_ij (/ dist_ij for
@@ -295,7 +295,7 @@ KGE_API int kge_ipc_open(kge_handle_t h, const uint8_t handle[64], int64_t offse
 /* Shard memory for LARGE tables (what dglke_b200.dist uses): CUDA virtual-memory-management allocations, shared between
  * the ranks as POSIX file descriptors (pass them over a Unix socket, SCM_RIGHTS) and mapped with 2 MiB pages on the owner
  * and on every peer.  kge_ipc_open maps a peer's cudaMalloc range with small pages, and random row reads over a shard of
- * tens of GB then miss the reader's TLB on every row (measured 340 us vs 60 us per 14 800 rows, tools/peer_gather_probe.py).
+ * tens of GB then miss the reader's TLB on every row.
  *   kge_shard_alloc   allocate `bytes` (rounded up to the mapping granularity) on the handle's device, map it read/write,
  *                     return the pointer and a file descriptor the caller passes to peers and then close()s
  *   kge_shard_import  map the allocation behind a received descriptor read/write on the handle's device (same `bytes`)

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY -- times the reference's CPU implementation of the step on the host cores: the UNMODIFIED
-reference's `KEModel.forward -> loss.backward() -> KEModel.update` when its package is installed under baseline/_ref
-(impl="reference"; `__graft_entry__.build()` pip-installs it there from /root/reference, git-ignored), else the CPU oracle
+reference's `KEModel.forward -> loss.backward() -> KEModel.update` when its package is installed under oracle/_ref
+(impl="reference"; `__graft_entry__.build()` pip-installs it there from $KGE_REFERENCE_PY, git-ignored), else the CPU oracle
 (oracle/kge_oracle.py, a port of the same PyTorch step; impl="port").  Both run under the reference's own process model:
 `num_proc` forked Hogwild workers sharing the tables through shared memory, one intra-op thread
 each, a barrier before and after (train.py:290-317, train_pytorch.py:255-259).  Sampling is
@@ -36,7 +36,7 @@ def make_batches(n_ent, n_rel, B, Ns, n_batches, seed):
     return out
 
 
-REF_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "baseline", "_ref")
+REF_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
 
 
 def reference_installed():

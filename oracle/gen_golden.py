@@ -1,5 +1,5 @@
-"""Generates tests/golden/*.npz from the UNMODIFIED reference (run in the build container,
-where /root/reference exists):   python oracle/gen_golden.py
+"""Generates tests/golden/*.npz from the UNMODIFIED reference (KGE_REFERENCE_PY names its
+python/ directory):   python oracle/gen_golden.py
 
 Every array in a fixture is an output of the reference's own code path
 (KEModel.forward -> loss.backward() -> KEModel.update, predict_neg_score) driven through
@@ -33,7 +33,7 @@ CASES.append(("TransE_l2_impts", "TransE_l2", dict(adv=True, impts=True)))
 # regularisation off / L2 regulariser
 CASES.append(("DistMult_noreg", "DistMult", dict(adv=False, reg_coef=0.0)))
 CASES.append(("ComplEx_reg2", "ComplEx", dict(adv=True, reg_norm=2, reg_coef=1e-3)))
-# tensor-core shapes (D >= 32, chunk / neg multiples of 8): the tcgen05 kernels are pinned against the reference directly
+# tensor-core shapes (D >= 32, chunk / neg multiples of 8): the tensor-core kernels are pinned against the reference directly
 CASES.append(("tc_TransE_l2_adv", "TransE_l2", dict(adv=True, hidden=32, batch=16, chunk=8, neg=8, n_ent=60)))
 CASES.append(("tc_TransE_l2_ragged_impts", "TransE_l2", dict(adv=True, hidden=40, batch=32, chunk=16, neg=8, n_ent=60, impts=True)))
 CASES.append(("tc_DistMult_uni", "DistMult", dict(adv=False, hidden=32, batch=16, chunk=8, neg=16, n_ent=60)))

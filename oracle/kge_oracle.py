@@ -4,14 +4,14 @@ A torch-fp32 CPU restatement of the per-step arithmetic of awslabs/dgl-ke
 (gather -> score over 1 positive + chunk-shared negatives -> logsigmoid /
 self-adversarial loss -> autograd -> row-sparse Adagrad).  It exists so that the
 parity tests, `__graft_entry__.smoke()` and `bench.py`'s `cpu_baseline` /
-`--impl reference` legs have a checker that travels to the GPU box (the reference
+`--impl reference` legs have a checker that needs nothing but torch (the reference
 tree itself does not).  NOTHING in the product path may import this module.
 
 Parity is PINNED: tests/test_oracle_golden.py checks every function below against
 fixtures in tests/golden/ that were produced by the *unmodified reference* driven by
 oracle/ref_harness.py (generator: oracle/gen_golden.py).
 
-Each function cites the reference lines (relative to /root/reference/python/dglke) it
+Each function cites the reference lines (relative to python/dglke of awslabs/dgl-ke) it
 follows.  Layout conventions (SURVEY.md Appendix A):
   * tables are fp32 row-major [num, dim]; indices int64
   * ComplEx rows are [re | im]; RotatE entity rows are [re | im], relation rows are phases

@@ -1,5 +1,5 @@
-"""TEST INFRASTRUCTURE ONLY -- drives the UNMODIFIED reference (awslabs/dgl-ke,
-/root/reference/python/dglke) on CPU torch so that golden vectors can be generated
+"""TEST INFRASTRUCTURE ONLY -- drives the UNMODIFIED reference (awslabs/dgl-ke; REFERENCE_PY below says
+where a checkout is looked for) on CPU torch so that golden vectors can be generated
 from the reference itself (SURVEY.md section 8c).
 
 The reference's hot path needs DGL only for (a) a dozen `dgl.backend` tensor aliases
@@ -8,7 +8,7 @@ the arithmetic that is recorded in tests/golden/ is executed by the reference's 
 `KEModel.forward` -> `loss.backward()` -> `KEModel.update()`
 (general_models.py:529-588, tensor_models.py:270-362, score_fun.py, loss.py:69-98).
 
-This file can only run where /root/reference exists (the build container).  Nothing in
+This file can only run where a checkout of the reference exists.  Nothing in
 the product, `-m gpu` tests, smoke() or bench.py imports it.
 """
 import os
@@ -19,7 +19,9 @@ import argparse
 import numpy as np
 import torch as th
 
-REFERENCE_PY = os.environ.get("KGE_REFERENCE_PY", "/root/reference/python")
+# python/ of a checkout of the reference: KGE_REFERENCE_PY, else a `reference` directory next to this repository
+REFERENCE_PY = os.path.abspath(os.environ.get("KGE_REFERENCE_PY") or os.path.join(
+    os.path.dirname(os.path.abspath(__file__)), "..", "..", "reference", "python"))
 
 
 def reference_available():

@@ -46,3 +46,20 @@ def tables_before(z, step):
         return ent, th.zeros(ent.shape[0]), rel, th.zeros(rel.shape[0])
     p = "s%d_" % (step - 1)
     return f(z[p + "ent_emb"]), f(z[p + "ent_state"]), f(z[p + "rel_emb"]), f(z[p + "rel_state"])
+
+
+REF_HOST = os.path.join(GOLDEN_DIR, "reference_host.json.gz")
+
+
+def reference_result(key, make):
+    """What the unmodified reference returned for `key` (dataset readers, parser tables): stored in
+    tests/golden/reference_host.json.gz.  With KGE_WRITE_GOLDEN=1 (and a checkout of the reference, see
+    oracle/ref_harness.py) make() is run on the reference instead: a new key is stored, an existing one must match."""
+    import gzip
+    db = json.load(gzip.open(REF_HOST, "rt")) if os.path.exists(REF_HOST) else {}
+    if os.environ.get("KGE_WRITE_GOLDEN") == "1":
+        data = json.loads(json.dumps(make()))
+        assert db.setdefault(key, data) == data, key
+        with gzip.GzipFile(REF_HOST, "wb", mtime=0) as f:
+            f.write(json.dumps(db, sort_keys=True).encode())
+    return db[key]

@@ -1,4 +1,4 @@
-"""Stress / determinism probe of the tcgen05 score GEMM (run manually on a B200):
+"""Stress / determinism probe of the wgmma score GEMM (run manually on an H100):
 repeats kge_score_neg on fresh random rows and compares with an fp64 evaluation of the same formula."""
 import os
 import sys

@@ -1,8 +1,8 @@
-"""Fused tcgen05 kernel (kge_fused.cu), stage by stage, against float64 evaluations of the reference formulas:
+"""Fused wgmma kernel (kge_fused.cu), stage by stage, against float64 evaluations of the reference formulas:
 
   stage 1  S = A.Bn^T (+ distance epilogue)        -> negative scores        (KGE_BUF_NEG_SCORE)
   stage 2  loss / softmax / backward coefficients   -> dL/dneg (/dist)        (kge_debug_set_dump, both passes)
-  stage 3  G = V.Y with V read from TMEM            -> negative / node grads  (KGE_BUF_NEG_GRAD, KGE_BUF_NODE_GRAD)
+  stage 3  G = V.Y with V as the register operand   -> negative / node grads  (KGE_BUF_NEG_GRAD, KGE_BUF_NODE_GRAD)
 
 and the 5-launch fused step (kge_step_fused) against the oracle's step.  A failure message says which stage broke."""
 import numpy as np
@@ -22,7 +22,7 @@ SHAPES = [  # (model, hidden, gamma, n_ent, n_rel, B, Cs, Ns, adv)
     ("TransE_l2", 96, 10.0, 977, 13, 320, 160, 72, True),            # ragged: Cs != Ns, two row tiles, D = 3 slab blocks
     ("DistMult", 40, 5.0, 500, 7, 96, 48, 24, True),                 # D not a multiple of 32
     ("TransE_l2", 400, 19.9, 14951, 1345, 6000, 200, 200, True),     # 60 tiles per pass
-    ("DistMult", 128, 12.0, 3000, 20, 48000, 240, 240, True),        # 400 tiles > 148 SMs: persistent loop, ring hand-over between tiles
+    ("DistMult", 128, 12.0, 3000, 20, 48000, 240, 240, True),        # 400 tiles > 132 SMs: persistent loop, ring hand-over between tiles
 ]
 
 
@@ -132,7 +132,7 @@ def test_fused_step_five_launches_matches_oracle(cfg):
 @pytest.mark.parametrize("model,hidden,de", [("TransE_l1", 64, False), ("RotatE", 32, True), ("RESCAL", 32, False),
                                              ("DistMult", 20, False)])
 def test_step_fused_schedule_with_the_tile_kernels(model, hidden, de):
-    """kge_step_fused on shapes / models the tcgen05 kernel does not take (L1, RotatE, RESCAL, D < 32): same fused-step
+    """kge_step_fused on shapes / models the wgmma kernel does not take (L1, RotatE, RESCAL, D < 32): same fused-step
     schedule (no node cache, dense relation sums, log scalars from the update kernel) over the fp32 tile kernels."""
     hp = ko.Hyper(model=model, hidden_dim=hidden, gamma=8.0, lr=0.1, reg_coef=1e-6, reg_norm=3, adversarial=True,
                   double_ent=de)
@@ -184,7 +184,7 @@ def test_fused_and_unfused_paths_agree():
 
 def test_fused_kernel_stress_200_runs():
     """200 back-to-back runs of the fused kernels on fresh random rows (hot chunk shape, both corruption modes): every
-    run's scores and both coefficient passes against float64.  A race in the TMA / mbarrier / TMEM hand-offs would show
+    run's scores and both coefficient passes against float64.  A race in the TMA / mbarrier / wgmma hand-offs would show
     up as sporadic garbage; this is the default engine's collected stress test (tests/stress_umma.py is the manual one
     for the stand-alone GEMMs)."""
     from dglke_b200 import _lib

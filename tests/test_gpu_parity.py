@@ -45,7 +45,7 @@ def _oracle_fp64(hp, tables, si, C, Cs, Ns):
 def _run_and_check(hp, tables, si, C, Cs, Ns, ref, tol=2e-5, allow_fp64_arbitration=True):
     """Runs one step on the GPU through the C ABI and compares every traced quantity with `ref` (numpy dict from
     the reference's golden vectors or from the fp32 CPU oracle).  If the fp32 oracle itself is the outlier -- the
-    CPU sgemm of the GPU boxes' AMX Xeons has been seen to lose precision sporadically -- the comparison is repeated
+    CPU sgemm of AMX Xeon hosts has been seen to lose precision sporadically -- the comparison is repeated
     against the same oracle evaluated in float64, with the SAME tolerances."""
     from dglke_b200 import _lib
     tables0 = [x.clone() for x in tables]

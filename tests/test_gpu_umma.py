@@ -1,4 +1,4 @@
-"""tcgen05 engine (engine=1: TMA + tcgen05.mma 3xTF32 + TMEM epilogues) against the CPU oracle, same
+"""wgmma engine (engine=1: TMA + wgmma 3xTF32 + register epilogues) against the CPU oracle, same
 tolerances as the fp32 tile engine -- the 3xTF32 split keeps fp32-level accuracy."""
 import numpy as np
 import pytest

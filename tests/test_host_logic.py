@@ -9,30 +9,34 @@ import torch as th
 
 from dglke_b200 import utils, graph
 
-REF = "/root/reference/python"
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_flag_surface_matches_reference_parser():
-    """Every option string, default and type of dglke_train's parser (utils.py:199-297, train.py:40-60)."""
-    if not os.path.isdir(os.path.join(REF, "dglke")):
-        pytest.skip("reference tree not present (GPU box)")
-    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle"))
-    import ref_harness as rh
-    rh.import_reference()
-    import importlib
-    ref_utils = importlib.import_module("dglke.utils")
-    ref_parser = ref_utils.CommonArgParser()
-    ours = utils.CommonArgParser()
+    """Every option string, default and type of dglke_train's parser (utils.py:199-297, train.py:40-60), against the
+    table read off the reference's own parser and stored under tests/golden (golden_util.reference_result)."""
+    import json
 
     def table(p):
-        return {tuple(a.option_strings): (a.default, a.type, a.nargs, tuple(a.choices) if a.choices else None,
-                                          type(a).__name__)
+        return {" ".join(a.option_strings): [a.default, a.type.__name__ if a.type else None, a.nargs,
+                                             list(a.choices) if a.choices else None, type(a).__name__]
                 for a in p._actions if a.option_strings and a.dest != "help"}
-    assert table(ours) == table(ref_parser)
-    # train-only flags (train.py:44-60): read from the source since importing dglke.train needs more of DGL
-    src = open(os.path.join(REF, "dglke", "train.py")).read()
-    for flag in ("--gpu", "--mix_cpu_gpu", "--valid", "--rel_part", "--async_update", "--has_edge_importance"):
-        assert flag in src
+    train_flags = ("--gpu", "--mix_cpu_gpu", "--valid", "--rel_part", "--async_update", "--has_edge_importance")
+
+    def from_reference():
+        sys.path.insert(0, os.path.join(ROOT, "oracle"))
+        import ref_harness as rh
+        rh.import_reference()
+        import importlib
+        ref_utils = importlib.import_module("dglke.utils")
+        # train-only flags (train.py:44-60): read from the source since importing dglke.train needs more of DGL
+        src = open(os.path.join(rh.REFERENCE_PY, "dglke", "train.py")).read()
+        return {"common": table(ref_utils.CommonArgParser()), "train_only": [f for f in train_flags if f in src]}
+    from golden_util import reference_result
+    want = reference_result("parser_flags", from_reference)
+    assert json.loads(json.dumps(table(utils.CommonArgParser()))) == want["common"]
+    assert want["train_only"] == list(train_flags)
+    for flag in train_flags:
         assert any(flag in a.option_strings for a in utils.ArgParser()._actions)
 
 

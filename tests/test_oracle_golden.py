@@ -1,4 +1,4 @@
-"""Pins oracle/kge_oracle.py (the CPU restatement that travels to the GPU box) against the
+"""Pins oracle/kge_oracle.py (the CPU restatement the GPU tests compare against) against the
 golden vectors produced by the unmodified reference (oracle/gen_golden.py).  CPU only."""
 import numpy as np
 import pytest
