@@ -321,8 +321,8 @@ BatchView bview(const kge_batch_t* b) {
 
 namespace kge {
 // RESCAL-specific row kernels (kge_rescal.cu)
-void launch_rescal_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
-                        const BatchView&, const StepWs&);
+cudaError_t launch_rescal_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
+                               const BatchView&, const StepWs&);
 void launch_rescal_prep_dense(const LaunchCtx&, const StepParams&, const float* head, const float* relr,
                               const float* tail, const StepWs&, bool want_pos, bool want_a);
 void launch_rescal_chain(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
@@ -668,8 +668,8 @@ static int forward_backward_impl(kge_handle_t h, const kge_step_cfg_t* cfg, cons
     }
   }
   if (p.use_nc && !p.nc_staged) launch_gather_nodes(c, p, ve, b, w);      // pos_g.ndata['emb'] = entity_emb(pos_g.ndata['id'])  (general_models.py:548)
-  if (p.model == KGE_RESCAL) launch_rescal_prep(c, p, ve, vr, b, w);
-  else launch_prep(c, p, ve, vr, b, w);
+  const cudaError_t pe = (p.model == KGE_RESCAL) ? launch_rescal_prep(c, p, ve, vr, b, w) : launch_prep(c, p, ve, vr, b, w);
+  if (pe != cudaSuccess) return fail(KGE_ERR_CUDA, "k_prep launch (d=%d): %s", p.D, cudaGetErrorString(pe));
   if (p.neg_deg) launch_negdeg_zero_reg(c, p, w);
   float* logdst = log4 ? log4 : h->dev_log4;
   if (p.fused) {

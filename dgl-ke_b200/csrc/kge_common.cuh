@@ -222,16 +222,25 @@ __device__ __forceinline__ long long slab_off(long long chunk, int nblk, int R, 
 __device__ __forceinline__ long long slabT_off(long long chunk, int R, int Ncol, int row, int col) {
   return ((chunk * slab_blocks(R) + (row >> 5)) * (long long)Ncol + col) * 32 + (row & 31);
 }
-// destination of an operand row: plain fp32 row-major and/or its TF32 hi/lo split in slab layout (+ transposed slabs)
+// k_prep stages 32 operand rows in shared memory to write their transposed slabs as whole lines (kge_rows.cu).  Row
+// stride (floats): >= D and = 4 (mod 32), so that both the float4 stores along a row (8 lanes = 128 contiguous bytes) and
+// the float4 loads of one column group by 8 consecutive rows (8 distinct 16-byte bank groups) are free of bank conflicts.
+constexpr int kPrepRows = 32;                         // = the row extent of one transposed slab block
+constexpr size_t kSmemOptinMax = 227 * 1024;          // per-block opt-in shared memory of sm_90
+__host__ __device__ inline int prep_stage_stride(int D) { return ((D + 27) & ~31) + 4; }
+inline size_t prep_stage_bytes(int D) { return (size_t)kPrepRows * prep_stage_stride(D) * sizeof(float); }
+// the wgmma engine (transposed slabs) is offered only where k_prep's staging buffer fits one CTA: D <= 1796
+inline bool prep_stage_fits(int D) { return prep_stage_bytes(D) <= kSmemOptinMax; }
+
+// destination of an operand row: plain fp32 row-major and/or its TF32 hi/lo split in slab layout, and/or a copy in
+// shared memory (k_prep writes the transposed slabs from there)
 struct RowOut {
   float* f32;        // row-major row pointer or null
   float* hi;         // slab-layout base pointers or null
   float* lo;
   long long chunk;
   int nblk, R, row;
-  float* hiT;        // transposed-slab base pointers or null
-  float* loT;
-  int D;             // row length (transposed slabs)
+  float* stage;      // shared-memory row or null
 };
 __device__ __forceinline__ void row_store4(const RowOut& o, int col, float4 v) {
   if (o.f32) *reinterpret_cast<float4*>(o.f32 + col) = v;
@@ -241,12 +250,8 @@ __device__ __forceinline__ void row_store4(const RowOut& o, int col, float4 v) {
     const long long off = slab_off(o.chunk, o.nblk, o.R, o.row, col);
     *reinterpret_cast<float4*>(o.hi + off) = h;
     *reinterpret_cast<float4*>(o.lo + off) = l;
-    if (o.hiT) {
-      const long long t = slabT_off(o.chunk, o.R, o.D, o.row, col);
-      o.hiT[t] = h.x; o.hiT[t + 32] = h.y; o.hiT[t + 64] = h.z; o.hiT[t + 96] = h.w;
-      o.loT[t] = l.x; o.loT[t + 32] = l.y; o.loT[t + 64] = l.z; o.loT[t + 96] = l.w;
-    }
   }
+  if (o.stage) *reinterpret_cast<float4*>(o.stage + col) = v;
 }
 
 // |x|^p  and  d/dx coef*|x|^p  (general_models.py:572-576: coef * norm(x, p)**p)
@@ -380,8 +385,8 @@ void launch_negdeg_zero_reg(const LaunchCtx&, const StepParams&, const StepWs&);
 void launch_negdeg_mask_scores(const LaunchCtx&, const StepParams&, const StepWs&);
 void launch_negdeg_mask_coef(const LaunchCtx&, const StepParams&, const StepWs&);
 void launch_negdeg_scatter(const LaunchCtx&, const StepParams&, const TableView& ent, const BatchView&, const StepWs&);   // row slots per prefetch warp the shape leaves room for (< 2: none)
-void launch_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
-                 const BatchView&, const StepWs&);
+cudaError_t launch_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
+                        const BatchView&, const StepWs&);
 // dense-row variant used by kge_score_pos / kge_score_neg (rows already gathered)
 void launch_prep_dense(const LaunchCtx&, const StepParams&, const float* head, const float* relr,
                        const float* tail, const float* negrows, const StepWs&, bool want_pos, bool want_a);

@@ -535,6 +535,7 @@ bool fused_supported(const StepParams& p) {
   if (!model_ok) return false;
   if (p.hinge || p.pairwise || p.neg_deg) return false;   // the fused epilogue is the plain (non-pairwise, unmasked) Logsigmoid criterion
   if ((p.D % 8) || (p.Cs % 8) || (p.Ns % 8) || p.D < 32 || p.Cs < 8 || p.Ns < 8) return false;
+  if (!prep_stage_fits(p.D)) return false;                  // the operand slabs come from k_prep's shared-memory staging
   return p.Cs <= 240 && p.Ns <= 240;
 }
 

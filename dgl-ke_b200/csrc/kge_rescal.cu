@@ -97,14 +97,14 @@ __global__ void __launch_bounds__(kBlock) k_rescal_fwd(StepParams p, const float
 }
 
 // generic neg / unique-node jobs of k_prep, shifted past the edge jobs (defined in kge_rows.cu)
-void launch_prep_nonedge(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
-                         const BatchView&, const StepWs&);
+cudaError_t launch_prep_nonedge(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
+                                const BatchView&, const StepWs&);
 
-void launch_rescal_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
-                        const BatchView& b, const StepWs& w) {
+cudaError_t launch_rescal_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
+                               const BatchView& b, const StepWs& w) {
   size_t smem = 4 * (size_t)p.D * sizeof(float);
   KGE_LAUNCH(c, k_rescal_fwd, (unsigned)p.B, kBlock, smem, p, nullptr, nullptr, nullptr, ent, rel, b, w, false, true, true);
-  launch_prep_nonedge(c, p, ent, rel, b, w);
+  return launch_prep_nonedge(c, p, ent, rel, b, w);
 }
 
 void launch_rescal_prep_dense(const LaunchCtx& c, const StepParams& p, const float* head, const float* relr,

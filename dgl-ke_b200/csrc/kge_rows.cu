@@ -178,60 +178,119 @@ __device__ __forceinline__ void edge_forward(const StepParams& p, const float* _
   else pos_out = s;
 }
 
-// Job space of k_prep: [0,B) edges | [B, B+Nn) negatives
+// Job space of k_prep: one CTA per (chunk, row block) -- C * ceil(Cs/rows) blocks of edge rows, then C * ceil(Ns/rows)
+// blocks of negative rows; the last block of a chunk may be partial.  One warp per row, lane -> columns as everywhere
+// else.  With the wgmma engine a block is 32 rows (4 per warp, one at a time): every row is also copied to shared
+// memory, and after a barrier the CTA writes the block's transposed slabs X^T[c][rb][col][0..31] from there: for each
+// column one warp store of 32 rows (lane = row) is one whole 128-byte line of hi and one of lo.  Written row by row,
+// each of those lines took 32 separate 4-byte stores.  Without transposed slabs (fp32 tiles) a block is 8 rows, one per
+// warp, so that small batches keep every row in flight at once.
+// The staging buffer (prep_stage_bytes, kge_common.cuh) is 52.5 KB at d = 400 and reaches the 227 KB a CTA may opt in
+// to at d = 1792; umma_supported / fused_supported keep larger rows on the fp32 tiles, which need no transposed slabs.
+__host__ __device__ inline int prep_block_rows(const StepWs& w) { return (w.AhiT || w.BhiT) ? kPrepRows : kWarpsPerBlock; }
+
+// KIT: slices per lane loaded ahead in the negatives' rows (1: local HBM, 4: sharded table).  Those are the only rows
+// k_prep may read over NVLink: with a sharded table the head / tail rows come from the local copy NC and the relation
+// table is replicated, so the edge rows always take edge_forward<MODEL, 1>, which keeps the kernel within 80 registers.
 template <int MODEL, int KIT>
-__global__ void __launch_bounds__(kRowBlock) k_prep(StepParams p, TableView ent, TableView rel, BatchView b, StepWs w,
-                                                     long long job0) {
-  long long job = job0 + (long long)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
+__global__ void __launch_bounds__(kRowBlock, 3) k_prep(StepParams p, TableView ent, TableView rel, BatchView b, StepWs w,
+                                                        int blk0) {
+  extern __shared__ float4 prep_stage_f4[];
+  float* const stage = reinterpret_cast<float*>(prep_stage_f4);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool reg_on = (p.reg_coef > 0.f && p.reg_norm > 0);
-  if (job < p.B) {
-    const float* h = head_row(p, ent, b, w, job);     // local copies made by k_gather_nodes, or table rows
-    const float* t = tail_row(p, ent, b, w, job);
-    const float* r = row_ptr(rel, b.rel_ids[job]);
-    float pos, a2, reg, nrm;
-    const long long ro = job * (long long)p.D;
-    // wgmma engine: A is only consumed as hi/lo operands; fp32 tiles: plain fp32
-    const RowOut ao{w.Ahi ? nullptr : w.A + ro, w.Ahi, w.Alo, job / p.Cs, slab_blocks(p.D), p.Cs, (int)(job % p.Cs), w.AhiT, w.AloT, p.D};
-    edge_forward<MODEL, KIT>(p, h, r, t, ao, lane, pos, a2, reg, nrm, true);
-    if (lane == 0) {
-      w.pos[job] = pos;
-      if (MODEL == KGE_TRANSE_L2) { w.a2[job] = a2; w.pnorm[job] = nrm; }
-      w.regp[job] = reg;
-    }
-    return;
-  }
-  job -= p.B;
-  if (job < p.Nn) {
-    const long long ro = job * (long long)p.D;
-    const float* src = w.BnRaw ? w.BnRaw + ro : row_ptr(ent, b.neg_ids[job]);   // staged by the previous step, or the table
-    // fused contraction: the negatives exist only as TF32 hi/lo slabs (Bn receives their gradient later)
-    const RowOut bo{p.fused ? nullptr : w.Bn + ro, w.Bhi, w.Blo, job / p.Ns, slab_blocks(p.D), p.Ns, (int)(job % p.Ns), w.BhiT, w.BloT, p.D};
-    float b2 = 0.f, reg = 0.f;
-    const int nv = p.D >> 2;
-    for (int v0 = 0; v0 < nv; v0 += kWarp * KIT) {
-      float4 x[KIT];
-#pragma unroll
-      for (int it = 0; it < KIT; ++it) {
-        const int v = v0 + lane + kWarp * it;
-        x[it] = (v < nv) ? ld4_stream(src + 4 * v) : make_float4(0.f, 0.f, 0.f, 0.f);
+  const int rows = prep_block_rows(w);
+  const int eblk = (p.Cs + rows - 1) / rows;
+  long long blk = (long long)blk0 + blockIdx.x;
+  const bool edge = blk < (long long)p.C * eblk;
+  if (!edge) blk -= (long long)p.C * eblk;
+  const int R = edge ? p.Cs : p.Ns, nblk = edge ? eblk : (p.Ns + rows - 1) / rows;
+  const long long chunk = blk / nblk;
+  const int rb = (int)(blk % nblk);
+  const int nrows = min(rows, R - rb * rows);
+  float* const hiT = edge ? w.AhiT : w.BhiT;
+  float* const loT = edge ? w.AloT : w.BloT;
+  const int S = prep_stage_stride(p.D);
+
+  for (int rl = warp; rl < nrows; rl += kWarpsPerBlock) {   // row within the block: a partial block keeps all warps busy
+    const int row = rb * rows + rl;
+    float* const st = hiT ? stage + rl * S : nullptr;
+    if (edge) {
+      const long long job = chunk * p.Cs + row;
+      const float* h = head_row(p, ent, b, w, job);     // local copies made by k_gather_nodes, or table rows
+      const float* t = tail_row(p, ent, b, w, job);
+      const float* r = row_ptr(rel, b.rel_ids[job]);
+      float pos, a2, reg, nrm;
+      // wgmma engine: A is only consumed as hi/lo operands; fp32 tiles: plain fp32
+      const RowOut ao{w.Ahi ? nullptr : w.A + job * (long long)p.D, w.Ahi, w.Alo, chunk, slab_blocks(p.D), p.Cs, row, st};
+      edge_forward<MODEL, 1>(p, h, r, t, ao, lane, pos, a2, reg, nrm, true);
+      if (lane == 0) {
+        w.pos[job] = pos;
+        if (MODEL == KGE_TRANSE_L2) { w.a2[job] = a2; w.pnorm[job] = nrm; }
+        w.regp[job] = reg;
       }
+    } else {
+      const long long job = chunk * p.Ns + row;
+      const long long ro = job * (long long)p.D;
+      const float* src = w.BnRaw ? w.BnRaw + ro : row_ptr(ent, b.neg_ids[job]);   // staged by the previous step, or the table
+      // fused contraction: the negatives exist only as TF32 hi/lo slabs (Bn receives their gradient later)
+      const RowOut bo{p.fused ? nullptr : w.Bn + ro, w.Bhi, w.Blo, chunk, slab_blocks(p.D), p.Ns, row, st};
+      float b2 = 0.f, reg = 0.f;
+      const int nv = p.D >> 2;
+      for (int v0 = 0; v0 < nv; v0 += kWarp * KIT) {
+        float4 x[KIT];
 #pragma unroll
-      for (int it = 0; it < KIT; ++it) {
-        const int v = v0 + lane + kWarp * it;
-        if (v >= nv) continue;
-        row_store4(bo, 4 * v, x[it]);
-        if (MODEL == KGE_TRANSE_L2) b2 += f4_dot(x[it], x[it]);
-        if (reg_on) reg += abs_pow4_sum(x[it], p.reg_norm);
+        for (int it = 0; it < KIT; ++it) {
+          const int v = v0 + lane + kWarp * it;
+          x[it] = (v < nv) ? ld4_stream(src + 4 * v) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int it = 0; it < KIT; ++it) {
+          const int v = v0 + lane + kWarp * it;
+          if (v >= nv) continue;
+          row_store4(bo, 4 * v, x[it]);
+          if (MODEL == KGE_TRANSE_L2) b2 += f4_dot(x[it], x[it]);
+          if (reg_on) reg += abs_pow4_sum(x[it], p.reg_norm);
+        }
+      }
+      b2 = warp_sum(b2); reg = warp_sum(reg);
+      if (lane == 0) {
+        if (MODEL == KGE_TRANSE_L2) w.b2[job] = b2;
+        w.regp[p.B + job] = reg;
       }
     }
-    b2 = warp_sum(b2); reg = warp_sum(reg);
-    if (lane == 0) {
-      if (MODEL == KGE_TRANSE_L2) w.b2[job] = b2;
-      w.regp[p.B + job] = reg;
-    }
-    return;
   }
+  if (!hiT) return;
+  __syncthreads();
+  // transposed slabs: warp `warp` takes column groups warp, warp + 8, ...; the padding rows of a partial block stay unwritten
+  if (lane >= nrows) return;
+  const long long base = ((chunk * nblk + rb) * (long long)p.D) * 32 + lane;
+  const float* srow = stage + lane * S;
+  for (int g = warp; g < (p.D >> 2); g += kWarpsPerBlock) {
+    float4 h, l;
+    split_tf32_4(*reinterpret_cast<const float4*>(srow + 4 * g), h, l);
+    float* dh = hiT + base + (long long)(4 * g) * 32;
+    float* dl = loT + base + (long long)(4 * g) * 32;
+    dh[0] = h.x; dh[32] = h.y; dh[64] = h.z; dh[96] = h.w;
+    dl[0] = l.x; dl[32] = l.y; dl[64] = l.z; dl[96] = l.w;
+  }
+}
+
+// dynamic shared memory of a k_prep launch (*bytes): the staging buffer exists only where the transposed slabs do; beyond
+// 48 KB (d > 356) the kernel has to opt in.  An error here means the launch must not be made.
+template <int MODEL, int KIT>
+cudaError_t prep_optin(const StepWs& w, int D, size_t* bytes) {
+  *bytes = (w.AhiT || w.BhiT) ? prep_stage_bytes(D) : 0;
+  if (*bytes > kSmemOptinMax) return cudaErrorInvalidValue;      // umma_supported keeps such rows off the wgmma engine
+  static size_t optin[64] = {};          // the opt-in shared-memory size is a per-device function attribute
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (*bytes > 48 * 1024 && dev >= 0 && dev < 64 && *bytes > optin[dev]) {
+    const cudaError_t e = cudaFuncSetAttribute(k_prep<MODEL, KIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*bytes);
+    if (e != cudaSuccess) return e;
+    optin[dev] = *bytes;
+  }
+  return cudaSuccess;
 }
 
 // ExternalEmbedding.__call__ on pos_g.ndata['id'] (general_models.py:548): NC[u,:] = ent[node_ids[u],:], one warp per
@@ -289,7 +348,7 @@ __global__ void __launch_bounds__(kRowBlock) k_prep_dense(StepParams p, const fl
     if (!want_pos) { if (p.neg_head) hrow = trow; else trow = hrow; }
     const long long ro = job * (long long)p.D;
     const RowOut ao{(want_a && !w.Ahi) ? w.A + ro : nullptr, want_a ? w.Ahi : nullptr, want_a ? w.Alo : nullptr,
-                    job / p.Cs, slab_blocks(p.D), p.Cs, (int)(job % p.Cs), nullptr, nullptr, p.D};
+                    job / p.Cs, slab_blocks(p.D), p.Cs, (int)(job % p.Cs), nullptr};
     edge_forward<MODEL, 1>(p, hrow, relr + job * (long long)p.Dr, trow, ao, lane, pos, a2, reg, nrm, want_a);
     if (lane == 0) {
       if (want_pos) w.pos[job] = pos;
@@ -301,7 +360,7 @@ __global__ void __launch_bounds__(kRowBlock) k_prep_dense(StepParams p, const fl
   if (job < p.Nn && negrows != nullptr) {
     const float* src = negrows + job * (long long)p.D;
     const long long ro = job * (long long)p.D;
-    const RowOut bo{nullptr, w.Bhi, w.Blo, job / p.Ns, slab_blocks(p.D), p.Ns, (int)(job % p.Ns), nullptr, nullptr, p.D};
+    const RowOut bo{nullptr, w.Bhi, w.Blo, job / p.Ns, slab_blocks(p.D), p.Ns, (int)(job % p.Ns), nullptr};
     float b2 = 0.f;
     for (int v = lane; v < (p.D >> 2); v += kWarp) {
       float4 x = ld4(src + 4 * v);
@@ -323,22 +382,33 @@ __global__ void __launch_bounds__(kRowBlock) k_prep_dense(StepParams p, const fl
     default: break;                                                         \
   }
 
-void launch_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
-                 const BatchView& b, const StepWs& w) {
-  long long jobs = p.B + p.Nn;
+cudaError_t launch_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
+                        const BatchView& b, const StepWs& w) {
+  const int rows = prep_block_rows(w);
+  const int blocks = p.C * (ceil_div(p.Cs, rows) + ceil_div(p.Ns, rows));
+  size_t smem = 0;
+  cudaError_t e = cudaSuccess;
   // sharded tables: deeper per-lane load batches hide the NVLink latency; local HBM prefers occupancy
   if (ent.n_shards > 1) {
-    KGE_DISPATCH_MODEL(p.model, KGE_LAUNCH(c, (k_prep<M, 4>), ceil_div(jobs, kWarpsPerBlock), kRowBlock, 0, p, ent, rel, b, w, 0LL));
+    KGE_DISPATCH_MODEL(p.model, if ((e = prep_optin<M, 4>(w, p.D, &smem)) == cudaSuccess)
+                                  KGE_LAUNCH(c, (k_prep<M, 4>), blocks, kRowBlock, smem, p, ent, rel, b, w, 0));
   } else {
-    KGE_DISPATCH_MODEL(p.model, KGE_LAUNCH(c, (k_prep<M, 1>), ceil_div(jobs, kWarpsPerBlock), kRowBlock, 0, p, ent, rel, b, w, 0LL));
+    KGE_DISPATCH_MODEL(p.model, if ((e = prep_optin<M, 1>(w, p.D, &smem)) == cudaSuccess)
+                                  KGE_LAUNCH(c, (k_prep<M, 1>), blocks, kRowBlock, smem, p, ent, rel, b, w, 0));
   }
+  return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-// negatives + unique-node jobs only (RESCAL runs its own per-edge kernel)
-void launch_prep_nonedge(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
-                         const BatchView& b, const StepWs& w) {
-  long long jobs = p.Nn;
-  KGE_LAUNCH(c, (k_prep<KGE_DISTMULT, 1>), ceil_div(jobs, kWarpsPerBlock), kRowBlock, 0, p, ent, rel, b, w, p.B);
+// the negatives' blocks only (RESCAL runs its own per-edge kernel)
+cudaError_t launch_prep_nonedge(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
+                                const BatchView& b, const StepWs& w) {
+  size_t smem = 0;
+  const cudaError_t e = prep_optin<KGE_DISTMULT, 1>(w, p.D, &smem);
+  if (e != cudaSuccess) return e;
+  const int rows = prep_block_rows(w);
+  KGE_LAUNCH(c, (k_prep<KGE_DISTMULT, 1>), p.C * ceil_div(p.Ns, rows), kRowBlock, smem, p, ent, rel, b, w,
+             p.C * ceil_div(p.Cs, rows));
+  return cudaGetLastError();
 }
 
 void launch_prep_dense(const LaunchCtx& c, const StepParams& p, const float* head, const float* relr,

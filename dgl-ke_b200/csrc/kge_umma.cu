@@ -274,7 +274,8 @@ bool tc_make_map(CUtensorMap* m, const float* base, long long rows, long long co
 
 bool umma_supported(const StepParams& p) {
   const bool model_ok = p.model == KGE_TRANSE_L2 || p.model == KGE_DISTMULT || p.model == KGE_COMPLEX || p.model == KGE_RESCAL;
-  return model_ok && (p.D % 8 == 0) && (p.Cs % 8 == 0) && (p.Ns % 8 == 0) && p.D >= 32 && p.Cs >= 8 && p.Ns >= 8;
+  return model_ok && (p.D % 8 == 0) && (p.Cs % 8 == 0) && (p.Ns % 8 == 0) && p.D >= 32 && p.Cs >= 8 && p.Ns >= 8 &&
+         prep_stage_fits(p.D);     // k_prep writes the transposed slabs from 32 rows staged in shared memory
 }
 
 namespace {
