@@ -12,19 +12,18 @@
 #include <cstdarg>
 #include <cstring>
 #include <cstdlib>
+#include <map>
+#include <mutex>
 #include <new>
+#include <utility>
 #include <cuda.h>
 #include "kge_common.cuh"
 
 namespace kge {
-bool umma_supported(const StepParams&);
-bool fused_supported(const StepParams&);
-}
-using namespace kge;
 
 namespace {
-
 thread_local char g_err[512] = "";
+}  // namespace
 
 int fail(int code, const char* fmt, ...) {
   va_list ap;
@@ -34,13 +33,70 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
+int smem_optin(const void* kernel, size_t bytes) {
+  if (bytes <= 48 * 1024) return KGE_OK;
+  // umma_supported keeps the shapes that would need more off the wgmma engine
+  if (bytes > kSmemOptinMax) return fail(KGE_ERR_UNSUPPORTED, "%zu bytes of shared memory per CTA requested, sm_90 allows %zu", bytes, kSmemOptinMax);
+  int dev = 0;
+  cudaGetDevice(&dev);
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> done;
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& have = done[{kernel, dev}];
+  if (bytes <= have) return KGE_OK;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(KGE_ERR_CUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize, %zu): %s", bytes, cudaGetErrorString(e));
+  }
+  have = bytes;
+  return KGE_OK;
+}
+
+// A buffer the library (re)allocates between steps: device memory, or page-locked host memory (the staging of
+// kge_step_fused_host).  The caller decides when and to what size.
+struct Buffer {
+  void* p = nullptr;
+  size_t bytes = 0;
+  bool host = false;
+  template <class T> T* as() const { return static_cast<T*>(p); }
+
+  void release() {
+    if (p) host ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr;
+    bytes = 0;
+  }
+  // Replaces the buffer by one of `n` bytes.  The old one may still be in use by work on `stream`, so this
+  // synchronises first, which a stream being captured into a CUDA graph must not do: there it refuses.
+  int resize(size_t n, cudaStream_t stream, const char* what) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaStreamIsCapturing(stream, &cs);
+    if (cs != cudaStreamCaptureStatusNone)
+      return fail(KGE_ERR_INVALID_ARG, "the %s must be (re)allocated (%zu bytes, has %zu) but the stream is capturing: "
+                  "run one eager step first", what, n, bytes);
+    cudaError_t e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return fail(KGE_ERR_CUDA, "cudaStreamSynchronize before reallocating the %s: %s", what, cudaGetErrorString(e));
+    release();
+    e = host ? cudaMallocHost(&p, n) : cudaMalloc(&p, n);
+    if (e != cudaSuccess) {
+      p = nullptr;
+      cudaGetLastError();
+      return fail(KGE_ERR_NOMEM, "%s(%zu) for the %s failed: %s", host ? "cudaMallocHost" : "cudaMalloc", n, what,
+                  cudaGetErrorString(e));
+    }
+    bytes = n;
+    return KGE_OK;
+  }
+};
+
+}  // namespace kge
+using namespace kge;
+
 #define KGE_CUDA_OK(expr)                                                                      \
   do {                                                                                         \
     cudaError_t e_ = (expr);                                                                   \
     if (e_ != cudaSuccess) return fail(KGE_ERR_CUDA, "%s: %s", #expr, cudaGetErrorString(e_)); \
   } while (0)
-
-}  // namespace
 
 struct kge_context {
   int device = 0;
@@ -48,24 +104,21 @@ struct kge_context {
   long long launches = 0;
   int engine = -1;
   int rel_deferred = 0;
-  // device arena (grown on demand, never inside a graph capture)
-  char* arena = nullptr;
-  size_t arena_bytes = 0;
+  // device arena of the step workspace (carve)
+  Buffer arena;
   // NG must be zero between steps: remember how much of it has been zeroed
   float* ng_ptr = nullptr;
   size_t ng_floats = 0;
   bool ng_dirty = false;   // a forward_backward whose gradients were never consumed by kge_update
   // pinned + device staging for the *_host entry points
-  char* pin = nullptr;
-  char* dev_stage = nullptr;
+  Buffer pin{nullptr, 0, true};
+  Buffer dev_stage;
   float* red_partial = nullptr;      // k_reduce_log partials + ticket + k_update barrier counters (persistent, zero-initialised once)
-  float* rel_dense = nullptr;        // [n_rel * Dr | n_rel] per-relation gradient sums of the fused step (zero between steps)
-  size_t rel_dense_floats = 0;
+  Buffer rel_dense;                  // [n_rel * Dr | n_rel] per-relation gradient sums of the fused step (zero between steps)
   float* ext_rg = nullptr;           // deferred relation mode: caller-owned dense buffers [n_rel * Dr], [n_rel] that k_chain sums
   float* ext_rgs = nullptr;          //   the relation gradients into (all-reduced by the caller, kge_set_relation_buffers)
   float* dump_v = nullptr;           // test hook (kge_debug_set_dump): coefficient matrices of the fused kernel
-  long long* negdeg_ids = nullptr;   // --neg_deg_sample: the augmented negative id list [C * (Cs + Ns)] of the last step
-  size_t negdeg_cap = 0;
+  Buffer negdeg_ids;                 // --neg_deg_sample: the augmented negative id list [C * (Cs + Ns)] of the last step
   // kge_set_next_batch: rows of the next step staged by this step's fused kernels
   struct Prefetch {
     bool armed = false;              // a next batch is registered for the coming kge_step_fused_begin
@@ -75,12 +128,53 @@ struct kge_context {
     const void *r_nodes = nullptr, *r_negs = nullptr, *r_nU_dev = nullptr;
     long long r_nU = 0, r_nneg = 0;
     int r_buf = 0;                   // which nc[] holds them
-    float* nc[2] = {nullptr, nullptr};
-    float* bn[2] = {nullptr, nullptr};  // double-buffered like nc: k_fused<N> of step k reads bn[cur] while it stages bn[cur^1]
-    size_t nc_floats = 0, bn_floats = 0;
+    Buffer nc[2];
+    Buffer bn[2];                    // double-buffered like nc: k_fused<N> of step k reads bn[cur] while it stages bn[cur^1]
+    FusedPrefetch args{};            // what this step's fused kernels copy
+
+    // `usable`: this step's fused kernels read rows from NC / BnRaw, so staged rows can stand in for its gathers.
+    // The rows the previous step staged replace this step's gathers -- only for exactly the batch that was announced.
+    void take_staged(const kge_batch_t& b, bool usable, StepParams& p, StepWs& w) {
+      if (!ready) return;
+      ready = false;
+      if (usable && r_nodes == b.node_ids && r_negs == b.neg_ids && r_nU == b.n_nodes &&
+          r_nU_dev == (b.n_nodes < 0 ? b.n_nodes_dev : nullptr) && r_nneg == p.Nn) {
+        w.NC = nc[r_buf].as<float>();
+        w.BnRaw = bn[r_buf].as<float>();
+        p.nc_staged = 1;
+      }
+    }
+
+    // Arms the copy of the announced next batch's rows by this step's fused kernels.  *out: what they copy, or null.
+    // `arena_nc`: the workspace's own NC, which this step falls back to when growing the buffers drops the staged rows.
+    int arm_next(bool usable, StepParams& p, StepWs& w, float* arena_nc, cudaStream_t stream, const FusedPrefetch** out) {
+      *out = nullptr;
+      if (!armed) return KGE_OK;
+      armed = false;
+      const long long ncap = 2 * p.B;
+      const long long nU = next.n_nodes < 0 ? ncap : next.n_nodes;
+      if (!usable || nU > ncap || next_nneg <= 0 || fused_prefetch_slots(p, 0) < 2 || fused_prefetch_slots(p, 1) < 2)
+        return KGE_OK;
+      const size_t ncb = (size_t)ncap * p.D * sizeof(float), bnb = (size_t)next_nneg * p.D * sizeof(float);
+      if (ncb > nc[0].bytes || ncb > nc[1].bytes || bnb > bn[0].bytes || bnb > bn[1].bytes) {
+        for (int i = 0; i < 2; ++i) {
+          int rc;
+          if ((rc = nc[i].resize(ncb, stream, "prefetch staging buffers")) || (rc = bn[i].resize(bnb, stream, "prefetch staging buffers")))
+            return rc;
+        }
+        w.BnRaw = nullptr; w.NC = arena_nc; p.nc_staged = 0;      // whatever was staged is gone with the old buffers
+      }
+      const int tgt = p.nc_staged ? (r_buf ^ 1) : 0;
+      const void* nU_dev = next.n_nodes < 0 ? next.n_nodes_dev : nullptr;
+      args = FusedPrefetch{(const long long*)next.node_ids, (const long long*)nU_dev, nU, (const long long*)next.neg_ids,
+                           next_nneg, nc[tgt].as<float>(), bn[tgt].as<float>()};
+      ready = true;
+      r_nodes = next.node_ids; r_negs = next.neg_ids; r_nU = next.n_nodes; r_nU_dev = nU_dev; r_nneg = next_nneg; r_buf = tgt;
+      *out = &args;
+      return KGE_OK;
+    }
   } pf;
   int fused_mode = -1;               // -1 default (fused kernel whenever the shape allows), 0 off
-  size_t stage_bytes = 0;
   float* dev_log4 = nullptr;
   // last step (for kge_update / kge_debug_read)
   StepParams last_p{};
@@ -131,7 +225,7 @@ int make_view(const kge_table_t* t, TableView* v, const char* what) {
   return KGE_OK;
 }
 
-int make_params(const kge_step_cfg_t* cfg, long long n_nodes, StepParams* p, bool need_tables) {
+int make_params(const kge_step_cfg_t* cfg, long long n_nodes, StepParams* p) {
   if (!cfg) return fail(KGE_ERR_INVALID_ARG, "cfg is null");
   if (cfg->model < KGE_TRANSE_L1 || cfg->model > KGE_ROTATE) return fail(KGE_ERR_INVALID_ARG, "unknown model %d", cfg->model);
   if (cfg->batch <= 0 || cfg->chunk_size <= 0 || cfg->neg_sample_size <= 0)
@@ -181,8 +275,6 @@ int make_params(const kge_step_cfg_t* cfg, long long n_nodes, StepParams* p, boo
   p->hinge = cfg->loss_genre == KGE_LOSS_HINGE ? 1 : 0;
   p->margin = cfg->margin;
   p->pairwise = cfg->pairwise ? 1 : 0;
-
-  (void)need_tables;
   return KGE_OK;
 }
 
@@ -201,90 +293,67 @@ bool use_fused(kge_context* h, const StepParams& p) {
   return h->engine != 0 && h->fused_mode != 0 && fused_supported(p);
 }
 
+bool use_umma(kge_context* h, const StepParams& p) {
+  return h->engine != 0 && umma_supported(p);    // engine -1 (default) / 1: wgmma whenever the shape allows it
+}
+
 int carve(kge_context* h, const StepParams& p, StepWs* w, cudaStream_t stream, const CarveOpt& opt = CarveOpt()) {
-  const size_t f = sizeof(float);
   const size_t BD = (size_t)p.B * p.D, ND = (size_t)p.Nn * p.D, BNs = (size_t)p.B * p.Ns;
-  const size_t U = (size_t)(p.U > 0 ? p.U : 0);
-  const bool rescal = p.model == KGE_RESCAL;
-  const bool um = !opt.force_tiles && (h->engine != 0) && umma_supported(p);
+  const size_t B = (size_t)p.B, Nn = (size_t)p.Nn, U = (size_t)(p.U > 0 ? p.U : 0);
+  const bool um = !opt.force_tiles && use_umma(h, p);
   const bool fused = p.fused != 0;
-  size_t need = 0;
-  auto take = [&](size_t floats) { size_t off = need; need += align_up(floats * f); return off; };
-  // NG first, sized for the largest possible node count (2B): rows >= U are never written, rows < U are
-  // re-zeroed by the node update, so one fill keeps the whole region zero across steps with varying U
-  size_t oNG = take((U ? (size_t)2 * p.B : 0) * p.D);
-  size_t oA = (um || fused) ? 0 : take(BD);
-  size_t oBn = take(ND), oGA = take(BD);
-  size_t oGR = p.rel_dense ? 0 : take((size_t)p.B * p.Dr);
-  size_t oS = (!fused || opt.want_scores) ? take(BNs) : 0;
-  size_t oV = fused ? 0 : take(BNs);
-  size_t opos = take(p.B), ogpos = take(p.B), opn = take(p.B), oa2 = take(p.B), ob2 = take(p.Nn);
-  size_t ors = take(p.B), ocs = take(p.Nn), opl = take(p.B), onl = take(p.B);
-  size_t owb = take(4), ogsr = take(p.B), ogsn = take(p.Nn), osm = take(p.B), osk = take(p.B);
-  size_t oMt = rescal ? take(BD) : 0;
   // slab layout pads the blocked dimension to a multiple of 32 (+ one slab of slack for box overruns)
-  const size_t sA = (size_t)p.B * slab_blocks(p.D) * 32 + 8192, sB = (size_t)p.Nn * slab_blocks(p.D) * 32 + 8192;
-  const size_t sV = (size_t)p.B * slab_blocks(p.Ns) * 32 + 8192;
-  size_t oAh = um ? take(sA) : 0, oAl = um ? take(sA) : 0, oBh = um ? take(sB) : 0, oBl = um ? take(sB) : 0;
-  size_t oVh = (um && !fused) ? take(sV) : 0, oVl = (um && !fused) ? take(sV) : 0;
+  const size_t sA = B * slab_blocks(p.D) * 32 + 8192, sB = Nn * slab_blocks(p.D) * 32 + 8192;
+  const size_t sV = B * slab_blocks(p.Ns) * 32 + 8192;
   // transposed slabs: [C][rows / 32][cols][32]
   const size_t sAT = (size_t)p.C * slab_blocks(p.Cs) * p.D * 32 + 8192, sBT = (size_t)p.C * slab_blocks(p.Ns) * p.D * 32 + 8192;
   const size_t sVT = (size_t)p.C * slab_blocks(p.Cs) * p.Ns * 32 + 8192;
-  size_t oAhT = um ? take(sAT) : 0, oAlT = um ? take(sAT) : 0, oBhT = um ? take(sBT) : 0, oBlT = um ? take(sBT) : 0;
-  size_t oVhT = (um && !fused) ? take(sVT) : 0, oVlT = (um && !fused) ? take(sVT) : 0;
-  // U-dependent tail
-  size_t oNC = p.use_nc ? take(U * p.D) : 0;
-  size_t oreg = take((size_t)p.B + p.Nn + (U ? (size_t)2 * p.B : 0));
-  if (need > h->arena_bytes) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(stream, &cs);
-    if (cs != cudaStreamCaptureStatusNone)
-      return fail(KGE_ERR_INVALID_ARG, "workspace must grow (%zu > %zu bytes) but the stream is capturing: run one eager step first", need, h->arena_bytes);
-    KGE_CUDA_OK(cudaStreamSynchronize(stream));
-    if (h->arena) KGE_CUDA_OK(cudaFree(h->arena));
-    h->arena = nullptr; h->arena_bytes = 0; h->ng_ptr = nullptr; h->ng_floats = 0;
-    size_t bytes = need + need / 4;
-    cudaError_t e = cudaMalloc(&h->arena, bytes);
-    if (e != cudaSuccess) { cudaGetLastError(); return fail(KGE_ERR_NOMEM, "cudaMalloc(%zu) for the step workspace failed: %s", bytes, cudaGetErrorString(e)); }
-    h->arena_bytes = bytes;
+  struct Slot { float** ptr; size_t floats; bool on; };
+  const Slot slots[] = {
+      // NG first, sized for the largest possible node count (2B): rows >= U are never written, rows < U are
+      // re-zeroed by the node update, so one fill keeps the whole region zero across steps with varying U
+      {&w->NG, (U ? 2 * B : 0) * p.D, true},
+      {&w->A, BD, !(um || fused)}, {&w->Bn, ND, true}, {&w->GA, BD, true}, {&w->GR, B * p.Dr, !p.rel_dense},
+      {&w->S, BNs, !fused || opt.want_scores}, {&w->V, BNs, !fused},
+      {&w->pos, B, true}, {&w->gpos, B, true}, {&w->pnorm, B, true}, {&w->a2, B, true}, {&w->b2, Nn, true},
+      {&w->rowsum, B, true}, {&w->colsum, Nn, true}, {&w->pl, B, true}, {&w->nl, B, true}, {&w->wbar, 4, true},
+      {&w->gsr, B, true}, {&w->gsn, Nn, true}, {&w->stat_m, B, true}, {&w->stat_k, B, true},
+      {&w->Mt, BD, p.model == KGE_RESCAL},
+      {&w->Ahi, sA, um}, {&w->Alo, sA, um}, {&w->Bhi, sB, um}, {&w->Blo, sB, um},
+      {&w->Vhi, sV, um && !fused}, {&w->Vlo, sV, um && !fused},
+      {&w->AhiT, sAT, um}, {&w->AloT, sAT, um}, {&w->BhiT, sBT, um}, {&w->BloT, sBT, um},
+      {&w->VhiT, sVT, um && !fused}, {&w->VloT, sVT, um && !fused},
+      // U-dependent tail
+      {&w->NC, U * p.D, p.use_nc != 0},
+      {&w->regp, B + Nn + (U ? 2 * B : 0), true},
+  };
+  size_t need = 0;
+  for (const Slot& s : slots)
+    if (s.on) need += align_up(s.floats * sizeof(float));
+  if (need > h->arena.bytes) {
+    if (int rc = h->arena.resize(need + need / 4, stream, "step workspace")) return rc;
+    h->ng_ptr = nullptr; h->ng_floats = 0;
   }
-  char* a = h->arena;
-  auto at = [&](size_t off, bool on) { return on ? (float*)(a + off) : nullptr; };
-  w->NG = (float*)(a + oNG); w->NC = at(oNC, p.use_nc != 0); w->A = at(oA, !(um || fused)); w->Bn = (float*)(a + oBn);
-  w->GA = (float*)(a + oGA); w->GR = at(oGR, !p.rel_dense); w->S = at(oS, !fused || opt.want_scores); w->V = at(oV, !fused);
-  w->pos = (float*)(a + opos); w->gpos = (float*)(a + ogpos); w->pnorm = (float*)(a + opn);
-  w->a2 = (float*)(a + oa2); w->b2 = (float*)(a + ob2); w->rowsum = (float*)(a + ors); w->colsum = (float*)(a + ocs);
-  w->pl = (float*)(a + opl); w->nl = (float*)(a + onl); w->regp = (float*)(a + oreg); w->wbar = (float*)(a + owb); w->gsr = (float*)(a + ogsr);
-  w->gsn = (float*)(a + ogsn); w->stat_m = (float*)(a + osm); w->stat_k = (float*)(a + osk);
+  size_t off = 0;
+  for (const Slot& s : slots) {
+    *s.ptr = s.on ? (float*)(h->arena.as<char>() + off) : nullptr;
+    if (s.on) off += align_up(s.floats * sizeof(float));
+  }
   w->red_partial = h->red_partial; w->red_ticket = (unsigned int*)(h->red_partial + 192);
   w->sync_ctr = (unsigned int*)(h->red_partial + 200);
   w->rg = nullptr; w->rgs = nullptr;
-  w->Mt = rescal ? (float*)(a + oMt) : nullptr;
-  w->Ahi = at(oAh, um); w->Alo = at(oAl, um); w->Bhi = at(oBh, um); w->Blo = at(oBl, um);
-  w->Vhi = at(oVh, um && !fused); w->Vlo = at(oVl, um && !fused);
-  w->AhiT = at(oAhT, um); w->AloT = at(oAlT, um); w->BhiT = at(oBhT, um); w->BloT = at(oBlT, um);
-  w->VhiT = at(oVhT, um && !fused); w->VloT = at(oVlT, um && !fused);
   return KGE_OK;
 }
 
 // dense per-relation gradient buffers of the fused single-GPU step (zero between steps: the update re-zeroes what it consumes)
 int ensure_rel_dense(kge_context* h, const TableView& rel, StepWs* w, cudaStream_t stream) {
-  const size_t need = (size_t)rel.num_rows * rel.dim + (size_t)rel.num_rows;
-  if (need != h->rel_dense_floats) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(stream, &cs);
-    if (cs != cudaStreamCaptureStatusNone)
-      return fail(KGE_ERR_INVALID_ARG, "relation gradient buffer must be (re)allocated but the stream is capturing: run one eager step first");
-    KGE_CUDA_OK(cudaStreamSynchronize(stream));
-    if (h->rel_dense) cudaFree(h->rel_dense);
-    h->rel_dense = nullptr; h->rel_dense_floats = 0;
-    cudaError_t e = cudaMalloc(&h->rel_dense, need * sizeof(float));
-    if (e != cudaSuccess) { cudaGetLastError(); return fail(KGE_ERR_NOMEM, "cudaMalloc(%zu) for the relation gradient sums failed", need * sizeof(float)); }
-    KGE_CUDA_OK(cudaMemsetAsync(h->rel_dense, 0, need * sizeof(float), stream));
-    h->rel_dense_floats = need;
+  const size_t bytes = ((size_t)rel.num_rows * rel.dim + (size_t)rel.num_rows) * sizeof(float);
+  if (bytes != h->rel_dense.bytes) {
+    if (int rc = h->rel_dense.resize(bytes, stream, "relation gradient sums")) return rc;
+    KGE_CUDA_OK(cudaMemsetAsync(h->rel_dense.p, 0, bytes, stream));
   }
-  w->rg = h->rel_dense;
-  w->rgs = h->rel_dense + (size_t)rel.num_rows * rel.dim;
+  w->rg = h->rel_dense.as<float>();
+  w->rgs = w->rg + (size_t)rel.num_rows * rel.dim;
   return KGE_OK;
 }
 
@@ -317,25 +386,13 @@ BatchView bview(const kge_batch_t* b) {
                    (const long long*)b->head_ids, (const long long*)b->tail_ids};
 }
 
-}  // namespace
+int run_score(kge_context* h, const LaunchCtx& c, const StepParams& p, const StepWs& w) {
+  if (use_umma(h, p)) return umma_score(c, p, w);
+  launch_score(c, p, w);
+  return KGE_OK;
+}
 
-namespace kge {
-// RESCAL-specific row kernels (kge_rescal.cu)
-cudaError_t launch_rescal_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
-                               const BatchView&, const StepWs&);
-void launch_rescal_prep_dense(const LaunchCtx&, const StepParams&, const float* head, const float* relr,
-                              const float* tail, const StepWs&, bool want_pos, bool want_a);
-void launch_rescal_chain(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
-                         const BatchView&, const StepWs&);
-// wgmma engine (kge_umma.cu): returns false when the shape is not handled (caller falls back to engine 0)
-bool umma_supported(const StepParams&);
-int umma_score(const LaunchCtx&, const StepParams&, const StepWs&, char* err, size_t errlen);
-int umma_grad(const LaunchCtx&, const StepParams&, const StepWs&, bool side_b, char* err, size_t errlen);
-// fused contraction (kge_fused.cu): mode 0 = P (scores, loss, GA), mode 1 = N (G_neg, mean squares)
-bool fused_supported(const StepParams&);
-int fused_launch(const LaunchCtx&, const StepParams&, const StepWs&, int mode, const float* wt, float* dumpS, float* dumpV,
-                 const TableView* ent, const long long* neg_ids, const FusedPrefetch* pf, char* err, size_t errlen);
-}  // namespace kge
+}  // namespace
 
 extern "C" {
 
@@ -376,14 +433,11 @@ KGE_API int kge_destroy(kge_handle_t h) {
   if (!h) return KGE_OK;
   DeviceGuard g(h->device);
   cudaDeviceSynchronize();
-  if (h->arena) cudaFree(h->arena);
-  if (h->dev_stage) cudaFree(h->dev_stage);
-  if (h->pin) cudaFreeHost(h->pin);
+  for (Buffer* b : {&h->arena, &h->dev_stage, &h->pin, &h->rel_dense, &h->negdeg_ids, &h->pf.nc[0], &h->pf.nc[1],
+                    &h->pf.bn[0], &h->pf.bn[1]})
+    b->release();
   if (h->dev_log4) cudaFree(h->dev_log4);
   if (h->red_partial) cudaFree(h->red_partial);
-  if (h->rel_dense) cudaFree(h->rel_dense);
-  if (h->negdeg_ids) cudaFree(h->negdeg_ids);
-  for (int i = 0; i < 2; ++i) { if (h->pf.nc[i]) cudaFree(h->pf.nc[i]); if (h->pf.bn[i]) cudaFree(h->pf.bn[i]); }
   if (h->prof.created)
     for (int i = 0; i < Profiler::kMax; ++i) { cudaEventDestroy(h->prof.ev0[i]); cudaEventDestroy(h->prof.ev1[i]); }
   delete h;
@@ -459,21 +513,6 @@ KGE_API int kge_gather(kge_handle_t h, const kge_table_t* table, const int64_t* 
   return KGE_OK;
 }
 
-static bool use_umma(kge_context* h, const StepParams& p) {
-  if (h->engine == 0) return false;   // engine -1 (default) / 1: wgmma whenever the shape allows it
-  return umma_supported(p);
-}
-
-static int run_score(kge_context* h, const LaunchCtx& c, const StepParams& p, const StepWs& w) {
-  if (use_umma(h, p)) {
-    int rc = umma_score(c, p, w, g_err, sizeof(g_err));
-    if (rc) return rc;
-  } else {
-    launch_score(c, p, w);
-  }
-  return KGE_OK;
-}
-
 KGE_API int kge_score_pos(kge_handle_t h, const kge_step_cfg_t* cfg, const float* head, const float* rel, const float* tail,
                   int64_t n, float* out, void* stream) {
   if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
@@ -484,7 +523,7 @@ KGE_API int kge_score_pos(kge_handle_t h, const kge_step_cfg_t* cfg, const float
   c2.batch = n; c2.chunk_size = (int32_t)1; c2.neg_sample_size = 1;
   if (n > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARG, "n too large");
   StepParams p;
-  int rc = make_params(&c2, 0, &p, false);
+  int rc = make_params(&c2, 0, &p);
   if (rc) return rc;
   DeviceGuard g(h->device);
   StepWs w{};
@@ -501,7 +540,7 @@ KGE_API int kge_score_neg(kge_handle_t h, const kge_step_cfg_t* cfg, const float
   if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
   if (!heads || !rel || !tails || !out) return fail(KGE_ERR_INVALID_ARG, "null pointer");
   StepParams p;
-  int rc = make_params(cfg, 0, &p, false);
+  int rc = make_params(cfg, 0, &p);
   if (rc) return rc;
   DeviceGuard g(h->device);
   StepWs w{};
@@ -534,7 +573,7 @@ KGE_API int kge_loss_grad(kge_handle_t h, const kge_step_cfg_t* cfg, const float
   if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
   if (!pos || !neg || !dpos || !dneg) return fail(KGE_ERR_INVALID_ARG, "null pointer");
   StepParams p;
-  int rc = make_params(cfg, 0, &p, false);
+  int rc = make_params(cfg, 0, &p);
   if (rc) return rc;
   p.model = KGE_DISTMULT;   // plain d loss / d score (no distance folding)
   DeviceGuard g(h->device);
@@ -571,7 +610,7 @@ static int forward_backward_impl(kge_handle_t h, const kge_step_cfg_t* cfg, cons
                                  const kge_batch_t* batch, float* log4, void* stream, bool fused_step) {
   if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
   StepParams p;
-  int rc = make_params(cfg, batch ? batch->n_nodes : 0, &p, true);
+  int rc = make_params(cfg, batch ? batch->n_nodes : 0, &p);
   if (rc) return rc;
   rc = check_batch(batch, p);
   if (rc) return rc;
@@ -599,84 +638,28 @@ static int forward_backward_impl(kge_handle_t h, const kge_step_cfg_t* cfg, cons
   BatchView b = bview(batch);
   if (p.neg_deg) {
     if (ve.n_shards != 1) return fail(KGE_ERR_UNSUPPORTED, "--neg_deg_sample needs a single-shard entity table");
-    if ((size_t)p.Nn > h->negdeg_cap) {
-      KGE_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
-      if (h->negdeg_ids) cudaFree(h->negdeg_ids);
-      h->negdeg_ids = nullptr; h->negdeg_cap = 0;
-      if (cudaMalloc(&h->negdeg_ids, (size_t)p.Nn * sizeof(long long)) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(KGE_ERR_NOMEM, "neg_deg_sample id list (%lld ids)", (long long)p.Nn);
-      }
-      h->negdeg_cap = (size_t)p.Nn;
-    }
-    launch_negdeg_ids(c, p, b, b.neg_ids, h->negdeg_ids);
-    b.neg_ids = h->negdeg_ids;          // from here on the step sees Cs + Ns ordinary negatives per chunk
+    const size_t bytes = (size_t)p.Nn * sizeof(long long);
+    if (bytes > h->negdeg_ids.bytes && (rc = h->negdeg_ids.resize(bytes, (cudaStream_t)stream, "neg_deg_sample id list")))
+      return rc;
+    launch_negdeg_ids(c, p, b, b.neg_ids, h->negdeg_ids.as<long long>());
+    b.neg_ids = h->negdeg_ids.as<long long>();          // from here on the step sees Cs + Ns ordinary negatives per chunk
   }
   ensure_ng_zero(h, p, w, c, false);
-  // rows staged by the previous step's prefetch warps (kge_set_next_batch) replace this step's gathers -- only for
-  // exactly the batch that was announced
-  auto& pf = h->pf;
+  // rows staged by the previous step's prefetch warps (kge_set_next_batch) are read by the fused kernels from NC / BnRaw
+  const bool stageable = fused_step && p.fused && p.use_nc;
   float* const arena_nc = w.NC;
-  if (pf.ready) {
-    const bool match = fused_step && p.fused && p.use_nc && pf.r_nodes == batch->node_ids && pf.r_negs == batch->neg_ids &&
-                       pf.r_nU == batch->n_nodes && pf.r_nU_dev == (batch->n_nodes < 0 ? batch->n_nodes_dev : nullptr) &&
-                       pf.r_nneg == p.Nn;
-    pf.ready = false;
-    if (match) { w.NC = pf.nc[pf.r_buf]; w.BnRaw = pf.bn[pf.r_buf]; p.nc_staged = 1; }
-  }
+  h->pf.take_staged(*batch, stageable, p, w);
   const FusedPrefetch* pfp = nullptr;
-  FusedPrefetch pfa{};
-  if (pf.armed) {
-    pf.armed = false;
-    const long long ncap = 2 * p.B;
-    const long long nU = pf.next.n_nodes < 0 ? ncap : pf.next.n_nodes;
-    if (fused_step && p.fused && p.use_nc && nU <= ncap && pf.next_nneg > 0 &&
-        fused_prefetch_slots(p, 0) >= 2 && fused_prefetch_slots(p, 1) >= 2) {
-      const size_t ncf = (size_t)ncap * p.D, bnf = (size_t)pf.next_nneg * p.D;
-      if (ncf > pf.nc_floats || bnf > pf.bn_floats) {
-        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-        cudaStreamIsCapturing((cudaStream_t)stream, &cs);
-        if (cs != cudaStreamCaptureStatusNone)
-          return fail(KGE_ERR_INVALID_ARG, "kge_set_next_batch: the staging buffers must exist before stream capture (run one eager step first)");
-        KGE_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
-        for (int i = 0; i < 2; ++i) {
-          if (pf.nc[i]) cudaFree(pf.nc[i]);
-          if (pf.bn[i]) cudaFree(pf.bn[i]);
-          pf.nc[i] = pf.bn[i] = nullptr;
-        }
-        pf.nc_floats = pf.bn_floats = 0;
-        if (cudaMalloc(&pf.nc[0], ncf * 4) != cudaSuccess || cudaMalloc(&pf.nc[1], ncf * 4) != cudaSuccess ||
-            cudaMalloc(&pf.bn[0], bnf * 4) != cudaSuccess || cudaMalloc(&pf.bn[1], bnf * 4) != cudaSuccess) {
-          cudaGetLastError();
-          return fail(KGE_ERR_NOMEM, "prefetch staging buffers (%zu MB)", (2 * ncf + 2 * bnf) * 4 >> 20);
-        }
-        pf.nc_floats = ncf; pf.bn_floats = bnf;
-        w.BnRaw = nullptr; w.NC = arena_nc; p.nc_staged = 0;      // whatever was staged is gone with the old buffers
-      }
-      const int tgt = p.nc_staged ? (pf.r_buf ^ 1) : 0;
-      pfa.node_ids = (const long long*)pf.next.node_ids;
-      pfa.nU_dev = pf.next.n_nodes < 0 ? (const long long*)pf.next.n_nodes_dev : nullptr;
-      pfa.nU = nU;
-      pfa.neg_ids = (const long long*)pf.next.neg_ids;
-      pfa.nNeg = pf.next_nneg;
-      pfa.nc = pf.nc[tgt]; pfa.bn = pf.bn[tgt];
-      pfp = &pfa;
-      pf.ready = true;
-      pf.r_nodes = pf.next.node_ids; pf.r_negs = pf.next.neg_ids; pf.r_nU = pf.next.n_nodes;
-      pf.r_nU_dev = pf.next.n_nodes < 0 ? pf.next.n_nodes_dev : nullptr;
-      pf.r_nneg = pf.next_nneg; pf.r_buf = tgt;
-    }
-  }
+  if ((rc = h->pf.arm_next(stageable, p, w, arena_nc, (cudaStream_t)stream, &pfp))) return rc;
   if (p.use_nc && !p.nc_staged) launch_gather_nodes(c, p, ve, b, w);      // pos_g.ndata['emb'] = entity_emb(pos_g.ndata['id'])  (general_models.py:548)
-  const cudaError_t pe = (p.model == KGE_RESCAL) ? launch_rescal_prep(c, p, ve, vr, b, w) : launch_prep(c, p, ve, vr, b, w);
-  if (pe != cudaSuccess) return fail(KGE_ERR_CUDA, "k_prep launch (d=%d): %s", p.D, cudaGetErrorString(pe));
+  if ((rc = (p.model == KGE_RESCAL) ? launch_rescal_prep(c, p, ve, vr, b, w) : launch_prep(c, p, ve, vr, b, w))) return rc;
   if (p.neg_deg) launch_negdeg_zero_reg(c, p, w);
   float* logdst = log4 ? log4 : h->dev_log4;
   if (p.fused) {
     launch_wbar(c, p, b.edge_weight, w);
-    if ((rc = fused_launch(c, p, w, 0, b.edge_weight, fused_step ? nullptr : w.S, h->dump_v, &ve, b.neg_ids, pfp, g_err, sizeof(g_err)))) return rc;
+    if ((rc = fused_launch(c, p, w, 0, b.edge_weight, fused_step ? nullptr : w.S, h->dump_v, &ve, b.neg_ids, pfp))) return rc;
     if ((rc = fused_launch(c, p, w, 1, b.edge_weight, nullptr,
-                           h->dump_v ? h->dump_v + (size_t)p.B * p.Ns : nullptr, &ve, b.neg_ids, pfp, g_err, sizeof(g_err)))) return rc;
+                           h->dump_v ? h->dump_v + (size_t)p.B * p.Ns : nullptr, &ve, b.neg_ids, pfp))) return rc;
   } else {
     if ((rc = run_score(h, c, p, w))) return rc;
     if (p.neg_deg) launch_negdeg_mask_scores(c, p, w);
@@ -685,8 +668,8 @@ static int forward_backward_impl(kge_handle_t h, const kge_step_cfg_t* cfg, cons
     if (p.neg_deg) launch_negdeg_mask_coef(c, p, w);
     launch_colsum(c, p, w);
     if (use_umma(h, p)) {
-      if ((rc = umma_grad(c, p, w, false, g_err, sizeof(g_err)))) return rc;
-      if ((rc = umma_grad(c, p, w, true, g_err, sizeof(g_err)))) return rc;
+      if ((rc = umma_grad(c, p, w, false))) return rc;
+      if ((rc = umma_grad(c, p, w, true))) return rc;
     } else {
       launch_grad_a(c, p, w);
       launch_grad_b(c, p, w);
@@ -714,7 +697,7 @@ static int update_impl(kge_handle_t h, const kge_step_cfg_t* cfg, const kge_tabl
   if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
   if (!h->have_last) return fail(KGE_ERR_INVALID_ARG, "kge_update without a preceding kge_forward_backward");
   StepParams p;
-  int rc = make_params(cfg, batch ? batch->n_nodes : 0, &p, true);
+  int rc = make_params(cfg, batch ? batch->n_nodes : 0, &p);
   if (rc) return rc;
   if ((rc = check_batch(batch, p))) return rc;
   if (p.B != h->last_p.B || p.Nn != h->last_p.Nn || p.U != h->last_p.U || p.model != h->last_p.model)
@@ -726,10 +709,8 @@ static int update_impl(kge_handle_t h, const kge_step_cfg_t* cfg, const kge_tabl
   StepParams q = h->last_p;       // the schedule flags (fused / use_nc / rel_dense / rel_deferred) of the forward pass
   q.lr = cfg->lr;
   BatchView b = bview(batch);
-  if (q.neg_deg) b.neg_ids = h->negdeg_ids;     // the list the forward pass built (Cs + Ns ids per chunk)
-  if (launch_update(lctx(h, stream), q, ve, vr, b, h->last_w, log4, b.edge_weight) != KGE_OK)
-    return fail(KGE_ERR_CUDA, "cooperative launch of k_update failed: %s (set KGE_B200_NO_COOP=1 for the three-launch form)",
-                cudaGetErrorString(cudaPeekAtLastError()));
+  if (q.neg_deg) b.neg_ids = h->negdeg_ids.as<long long>();     // the list the forward pass built (Cs + Ns ids per chunk)
+  if ((rc = launch_update(lctx(h, stream), q, ve, vr, b, h->last_w, log4, b.edge_weight))) return rc;
   KGE_CUDA_OK(cudaGetLastError());
   h->ng_dirty = false;
   h->have_last = false;   // gradients consumed (NG re-zeroed, like `self.trace = []`, tensor_models.py:362)
@@ -788,67 +769,48 @@ KGE_API int kge_step_fused_host(kge_handle_t h, const kge_step_cfg_t* cfg, const
   cudaStream_t st = (cudaStream_t)stream;
   const long long B = cfg->batch, Nn = B / cfg->chunk_size * cfg->neg_sample_size, U = bh->n_nodes;
   if (U <= 0 || U > 2 * B) return fail(KGE_ERR_INVALID_ARG, "n_nodes out of range");
-  const size_t n64 = (size_t)(U + 3 * B + Nn);
-  const size_t bytes = align_up(n64 * 8) + align_up(bh->edge_weight ? (size_t)B * 4 : 0) + 256;
-  if (bytes > h->stage_bytes) {
-    KGE_CUDA_OK(cudaStreamSynchronize(st));
-    if (h->pin) cudaFreeHost(h->pin);
-    if (h->dev_stage) cudaFree(h->dev_stage);
-    h->pin = nullptr; h->dev_stage = nullptr; h->stage_bytes = 0;
-    size_t cap = bytes + bytes / 2;
-    if (cudaMallocHost(&h->pin, cap) != cudaSuccess) { cudaGetLastError(); return fail(KGE_ERR_NOMEM, "cudaMallocHost(%zu) failed", cap); }
-    if (cudaMalloc(&h->dev_stage, cap) != cudaSuccess) { cudaGetLastError(); return fail(KGE_ERR_NOMEM, "cudaMalloc(%zu) failed", cap); }
-    h->stage_bytes = cap;
+  // staging layout: node_ids [U] | head_local, tail_local, rel_ids [B] | neg_ids [Nn] | 256-byte aligned edge_weight [B]
+  const void* src[6] = {bh->node_ids, bh->head_local, bh->tail_local, bh->rel_ids, bh->neg_ids, bh->edge_weight};
+  const size_t len[6] = {(size_t)U * 8, (size_t)B * 8, (size_t)B * 8, (size_t)B * 8, (size_t)Nn * 8,
+                         bh->edge_weight ? (size_t)B * 4 : 0};
+  size_t off[6] = {0};
+  for (int i = 1; i < 5; ++i) off[i] = off[i - 1] + len[i - 1];
+  off[5] = align_up(off[4] + len[4]);
+  const size_t end = len[5] ? off[5] + len[5] : off[4] + len[4];
+  const size_t bytes = off[5] + align_up(len[5]) + 256;
+  if (bytes > h->dev_stage.bytes) {
+    int rc;
+    if ((rc = h->pin.resize(bytes + bytes / 2, st, "host staging buffer")) ||
+        (rc = h->dev_stage.resize(bytes + bytes / 2, st, "device staging buffer")))
+      return rc;
   }
-  long long* pd = (long long*)h->dev_stage;
-  kge_batch_t bd{};
+  char* const dev = h->dev_stage.as<char>();
   // Fast path: the caller's arrays are page-locked (e.g. torch pinned tensors) -> DMA straight from them.
   auto is_pinned = [](const void* p) {
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
     return a.type == cudaMemoryTypeHost;
   };
-  const bool direct = is_pinned(bh->node_ids) && is_pinned(bh->head_local) && is_pinned(bh->tail_local) &&
-                      is_pinned(bh->rel_ids) && is_pinned(bh->neg_ids) && (!bh->edge_weight || is_pinned(bh->edge_weight));
-  size_t o = 0;
+  bool direct = true;
+  for (int i = 0; i < 6 && direct; ++i) direct = !len[i] || is_pinned(src[i]);
   if (direct) {
-    auto put = [&](const int64_t* src, long long n) -> const int64_t* {
-      const int64_t* d = (const int64_t*)(pd + o);
-      cudaMemcpyAsync(pd + o, src, (size_t)n * 8, cudaMemcpyHostToDevice, st);
-      o += (size_t)n;
-      return d;
-    };
-    bd.node_ids = put(bh->node_ids, U); bd.n_nodes = U;
-    bd.head_local = put(bh->head_local, B);
-    bd.tail_local = put(bh->tail_local, B);
-    bd.rel_ids = put(bh->rel_ids, B);
-    bd.neg_ids = put(bh->neg_ids, Nn);
-    if (bh->edge_weight) {
-      size_t woff = align_up(n64 * 8);
-      cudaMemcpyAsync(h->dev_stage + woff, bh->edge_weight, (size_t)B * 4, cudaMemcpyHostToDevice, st);
-      bd.edge_weight = (const float*)(h->dev_stage + woff);
-    }
+    for (int i = 0; i < 6; ++i)
+      if (len[i]) cudaMemcpyAsync(dev + off[i], src[i], len[i], cudaMemcpyHostToDevice, st);
     KGE_CUDA_OK(cudaGetLastError());
   } else {
     // the previous step's H2D copy must have drained before the library's pinned buffer is overwritten
     KGE_CUDA_OK(cudaStreamSynchronize(st));
-    long long* ph = (long long*)h->pin;
-    auto put = [&](const int64_t* src, long long n) { memcpy(ph + o, src, (size_t)n * 8); const int64_t* d = (const int64_t*)(pd + o); o += (size_t)n; return d; };
-    bd.node_ids = put(bh->node_ids, U); bd.n_nodes = U;
-    bd.head_local = put(bh->head_local, B);
-    bd.tail_local = put(bh->tail_local, B);
-    bd.rel_ids = put(bh->rel_ids, B);
-    bd.neg_ids = put(bh->neg_ids, Nn);
-    size_t wbytes = 0;
-    if (bh->edge_weight) {
-      size_t woff = align_up(n64 * 8);
-      memcpy(h->pin + woff, bh->edge_weight, (size_t)B * 4);
-      bd.edge_weight = (const float*)(h->dev_stage + woff);
-      wbytes = woff + (size_t)B * 4;
-    }
-    size_t copy_bytes = bh->edge_weight ? wbytes : n64 * 8;
-    KGE_CUDA_OK(cudaMemcpyAsync(h->dev_stage, h->pin, copy_bytes, cudaMemcpyHostToDevice, st));
+    for (int i = 0; i < 6; ++i)
+      if (len[i]) memcpy(h->pin.as<char>() + off[i], src[i], len[i]);
+    KGE_CUDA_OK(cudaMemcpyAsync(dev, h->pin.p, end, cudaMemcpyHostToDevice, st));
   }
+  kge_batch_t bd{};
+  bd.node_ids = (const int64_t*)(dev + off[0]); bd.n_nodes = U;
+  bd.head_local = (const int64_t*)(dev + off[1]);
+  bd.tail_local = (const int64_t*)(dev + off[2]);
+  bd.rel_ids = (const int64_t*)(dev + off[3]);
+  bd.neg_ids = (const int64_t*)(dev + off[4]);
+  bd.edge_weight = len[5] ? (const float*)(dev + off[5]) : nullptr;
   int rc = kge_step_fused(h, cfg, ent, rel, &bd, h->dev_log4, stream);
   if (rc) return rc;
   if (log4_host) KGE_CUDA_OK(cudaMemcpyAsync(log4_host, h->dev_log4, 4 * sizeof(float), cudaMemcpyDeviceToHost, st));

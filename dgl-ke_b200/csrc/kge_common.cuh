@@ -296,7 +296,17 @@ __device__ __forceinline__ float sigmoidf(float s) {
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // ------------------------------------------------------------------------------------------
-// host-side launchers (defined in kge_rows.cu / kge_tiles.cu / kge_rescal.cu)
+// host-side launchers and engines
+//
+// Errors: every host function that returns an int returns a KGE_* code and, when it is not KGE_OK, has already set the
+// message kge_last_error() returns (fail(), kge_abi.cu).  The void launchers only enqueue a kernel; their launch errors
+// are picked up by the caller's cudaGetLastError.
+int fail(int code, const char* fmt, ...);
+// Opts `kernel` in to `bytes` of dynamic shared memory on the current device when that exceeds the 48 KB default.  The
+// attribute belongs to the (kernel, device) pair; the largest size set so far is remembered, so only a larger size
+// costs a driver call.
+int smem_optin(const void* kernel, size_t bytes);
+
 // Optional per-launch timing (kge_profile_*): CUDA events recorded on the launching stream
 // around every kernel of a step; read back after a stream sync.
 struct Profiler {
@@ -366,26 +376,13 @@ struct SamplerParams {
 
 void launch_sampler(const LaunchCtx&, const SamplerParams&, long long step);
 
+// row kernels (kge_rows.cu, kge_tiles.cu)
 void launch_gather(const LaunchCtx&, const TableView& t, const long long* idx, long long n, float* out);
 void launch_gather_nodes(const LaunchCtx&, const StepParams&, const TableView& ent, const BatchView&, const StepWs&);
-// Rows of the NEXT step that the fused kernel's spare warps copy while it computes (kge_set_next_batch)
-struct FusedPrefetch {
-  const long long* node_ids;   // next batch's unique nodes
-  const long long* nU_dev;     // their count on the device, or null
-  long long nU;                // their count (capacity when nU_dev is set)
-  const long long* neg_ids;
-  long long nNeg;
-  float* nc;                   // [nU, D] destination of the node rows
-  float* bn;                   // [nNeg, D] destination of the negative rows
-};
-int fused_prefetch_slots(const StepParams& p, int mode);
-// --neg_deg_sample fix-up kernels (kge_negdeg.cu)
-void launch_negdeg_ids(const LaunchCtx&, const StepParams&, const BatchView&, const long long* sampled, long long* out);
-void launch_negdeg_zero_reg(const LaunchCtx&, const StepParams&, const StepWs&);
-void launch_negdeg_mask_scores(const LaunchCtx&, const StepParams&, const StepWs&);
-void launch_negdeg_mask_coef(const LaunchCtx&, const StepParams&, const StepWs&);
-void launch_negdeg_scatter(const LaunchCtx&, const StepParams&, const TableView& ent, const BatchView&, const StepWs&);   // row slots per prefetch warp the shape leaves room for (< 2: none)
-cudaError_t launch_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
+int launch_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
+                const BatchView&, const StepWs&);
+// k_prep's negative-row blocks only (RESCAL computes its edge rows in its own kernel)
+int launch_prep_nonedge(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
                         const BatchView&, const StepWs&);
 // dense-row variant used by kge_score_pos / kge_score_neg (rows already gathered)
 void launch_prep_dense(const LaunchCtx&, const StepParams&, const float* head, const float* relr,
@@ -411,5 +408,42 @@ void launch_node_grad_with_reg(const LaunchCtx&, const StepParams&, const TableV
 void launch_fill_zero(const LaunchCtx&, float* p, long long n);
 void launch_rel_grad_dense(const LaunchCtx&, const StepParams&, const BatchView&, const StepWs&, float* rg, float* rgs);
 void launch_rel_apply_dense(const LaunchCtx&, const TableView& rel, float* rg, float* rgs, float lr);
+
+// --neg_deg_sample fix-up kernels (kge_negdeg.cu)
+void launch_negdeg_ids(const LaunchCtx&, const StepParams&, const BatchView&, const long long* sampled, long long* out);
+void launch_negdeg_zero_reg(const LaunchCtx&, const StepParams&, const StepWs&);
+void launch_negdeg_mask_scores(const LaunchCtx&, const StepParams&, const StepWs&);
+void launch_negdeg_mask_coef(const LaunchCtx&, const StepParams&, const StepWs&);
+void launch_negdeg_scatter(const LaunchCtx&, const StepParams&, const TableView& ent, const BatchView&, const StepWs&);
+
+// RESCAL-specific row kernels (kge_rescal.cu)
+int launch_rescal_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
+                       const BatchView&, const StepWs&);
+void launch_rescal_prep_dense(const LaunchCtx&, const StepParams&, const float* head, const float* relr,
+                              const float* tail, const StepWs&, bool want_pos, bool want_a);
+void launch_rescal_chain(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
+                         const BatchView&, const StepWs&);
+
+// wgmma engine (kge_umma.cu): the three contractions as stand-alone GEMMs, for the shapes umma_supported accepts
+bool umma_supported(const StepParams&);
+int umma_score(const LaunchCtx&, const StepParams&, const StepWs&);
+int umma_grad(const LaunchCtx&, const StepParams&, const StepWs&, bool side_b);
+
+// fused contraction (kge_fused.cu): mode 0 = P (scores, loss, GA), mode 1 = N (G_neg, mean squares)
+// Rows of the NEXT step that the fused kernel's spare warps copy while it computes (kge_set_next_batch)
+struct FusedPrefetch {
+  const long long* node_ids;   // next batch's unique nodes
+  const long long* nU_dev;     // their count on the device, or null
+  long long nU;                // their count (capacity when nU_dev is set)
+  const long long* neg_ids;
+  long long nNeg;
+  float* nc;                   // [nU, D] destination of the node rows
+  float* bn;                   // [nNeg, D] destination of the negative rows
+};
+bool fused_supported(const StepParams&);
+// row slots per prefetch warp the shape leaves room for (< 2: none)
+int fused_prefetch_slots(const StepParams& p, int mode);
+int fused_launch(const LaunchCtx&, const StepParams&, const StepWs&, int mode, const float* wt, float* dumpS, float* dumpV,
+                 const TableView* ent, const long long* neg_ids, const FusedPrefetch* pf);
 
 }  // namespace kge

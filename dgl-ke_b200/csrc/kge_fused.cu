@@ -530,13 +530,9 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
 
 // The fused kernel keeps a whole row of the chunk's score matrix in the accumulator registers of one warpgroup
 // (columns / 2 registers per thread, next to the 64 of a GEMM2 chunk): at most 240 columns.
+// Its operands are those of the wgmma engine, and its epilogue is the plain (non-pairwise, unmasked) Logsigmoid criterion.
 bool fused_supported(const StepParams& p) {
-  const bool model_ok = p.model == KGE_TRANSE_L2 || p.model == KGE_DISTMULT || p.model == KGE_COMPLEX || p.model == KGE_RESCAL;
-  if (!model_ok) return false;
-  if (p.hinge || p.pairwise || p.neg_deg) return false;   // the fused epilogue is the plain (non-pairwise, unmasked) Logsigmoid criterion
-  if ((p.D % 8) || (p.Cs % 8) || (p.Ns % 8) || p.D < 32 || p.Cs < 8 || p.Ns < 8) return false;
-  if (!prep_stage_fits(p.D)) return false;                  // the operand slabs come from k_prep's shared-memory staging
-  return p.Cs <= 240 && p.Ns <= 240;
+  return umma_supported(p) && !p.hinge && !p.pairwise && !p.neg_deg && p.Cs <= 240 && p.Ns <= 240;
 }
 
 // mode 0 (P): S = A.Bn^T -> loss, coefficients -> GA;  mode 1 (N): S^T -> coefficients -> G_neg (+ mean square)
@@ -572,21 +568,15 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
 }
 
 template <int MODE, int NV>
-cudaError_t launch_variant(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
-  static bool attr_set[64] = {};          // the opt-in shared-memory size is a per-device function attribute
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_fused<MODE, NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    attr_set[dev] = true;
-  }
+int launch_variant(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+  if (int rc = smem_optin((const void*)k_fused<MODE, NV>, smem)) return rc;
   KGE_LAUNCH_NAMED(c, MODE == F_P ? "k_fused<P: S=A.Bn^T, loss, GA=V.Bn>" : "k_fused<N: S^T, G_neg=V^T.A, mean sq>",
                    (k_fused<MODE, NV>), grid, kThreadsF, smem, m[0], m[1], m[2], m[3], m[4], m[5], g);
-  return cudaGetLastError();
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? KGE_OK : fail(KGE_ERR_CUDA, "k_fused launch: %s", cudaGetErrorString(e));
 }
 template <int MODE>
-cudaError_t launch_width(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+int launch_width(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
   switch (g.N1) {
     case 64: return launch_variant<MODE, 64>(c, grid, smem, m, g);
     case 128: return launch_variant<MODE, 128>(c, grid, smem, m, g);
@@ -599,7 +589,7 @@ cudaError_t launch_width(const LaunchCtx& c, int grid, size_t smem, const CUtens
 int fused_prefetch_slots(const StepParams& p, int mode) { return geometry(p, mode, true).pf_slots; }
 
 int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int mode, const float* wt, float* dumpS,
-                 float* dumpV, const TableView* ent, const long long* neg_ids, const FusedPrefetch* pf, char* err, size_t errlen) {
+                 float* dumpV, const TableView* ent, const long long* neg_ids, const FusedPrefetch* pf) {
   FusedArgs g{};
   g.model = p.model; g.adversarial = p.adversarial;
   g.gamma = p.gamma; g.Tl2e = p.adv_temperature * kLog2e; g.inv2B = 0.5f / (float)p.B; g.uni = 1.f / (float)p.Ns;
@@ -607,7 +597,7 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
   g.C = p.C; g.D = p.D; g.nblkD = slab_blocks(p.D);
   const bool P = mode == 0;
   const Geometry q = geometry(p, mode, pf != nullptr && ent != nullptr);
-  if (!q.ok) { snprintf(err, errlen, "fused kernel: shape does not fit (N1=%d)", q.N1); return KGE_ERR_UNSUPPORTED; }
+  if (!q.ok) return fail(KGE_ERR_UNSUPPORTED, "fused kernel: shape does not fit (N1=%d)", q.N1);
   g.Rx = q.Rx; g.Ry = q.Ry; g.N1 = q.N1; g.nS1 = q.nS1; g.nS2 = q.nS2;
   g.stage1Bytes = q.stage1Bytes; g.stage2Bytes = q.stage2Bytes;
   if (pf && ent && q.pf_slots >= 2) {
@@ -636,17 +626,15 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
   const long long rowsX = (long long)p.C * g.Rx * g.nblkD, rowsY = (long long)p.C * g.Ry * g.nblkD;
   const long long rowsYT = (long long)p.C * slab_blocks(g.Ry) * g.D;
   CUtensorMap m[6];
-  if (!tc_make_map(&m[0], Xh, rowsX, 32, kTileM, err, errlen) || !tc_make_map(&m[1], Xl, rowsX, 32, kTileM, err, errlen) ||
-      !tc_make_map(&m[2], Yh, rowsY, 32, g.N1, err, errlen) || !tc_make_map(&m[3], Yl, rowsY, 32, g.N1, err, errlen) ||
-      !tc_make_map(&m[4], YhT, rowsYT, 32, kWc, err, errlen) || !tc_make_map(&m[5], YlT, rowsYT, 32, kWc, err, errlen))
+  if (tc_make_map(&m[0], Xh, rowsX, 32, kTileM) || tc_make_map(&m[1], Xl, rowsX, 32, kTileM) ||
+      tc_make_map(&m[2], Yh, rowsY, 32, g.N1) || tc_make_map(&m[3], Yl, rowsY, 32, g.N1) ||
+      tc_make_map(&m[4], YhT, rowsYT, 32, kWc) || tc_make_map(&m[5], YlT, rowsYT, 32, kWc))
     return KGE_ERR_CUDA;
   const size_t smem = kRingBytes + 1024;
   const int mtiles = (g.Rx + kTileM - 1) / kTileM;
   int grid = p.C * mtiles;
   if (grid > c.num_sms) grid = c.num_sms;
-  cudaError_t e = P ? launch_width<F_P>(c, grid, smem, m, g) : launch_width<F_N>(c, grid, smem, m, g);
-  if (e != cudaSuccess) { snprintf(err, errlen, "k_fused launch: %s", cudaGetErrorString(e)); return KGE_ERR_CUDA; }
-  return KGE_OK;
+  return P ? launch_width<F_P>(c, grid, smem, m, g) : launch_width<F_N>(c, grid, smem, m, g);
 }
 
 }  // namespace kge

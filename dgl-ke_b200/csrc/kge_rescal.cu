@@ -96,12 +96,9 @@ __global__ void __launch_bounds__(kBlock) k_rescal_fwd(StepParams p, const float
   }
 }
 
-// generic neg / unique-node jobs of k_prep, shifted past the edge jobs (defined in kge_rows.cu)
-cudaError_t launch_prep_nonedge(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
-                                const BatchView&, const StepWs&);
-
-cudaError_t launch_rescal_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
-                               const BatchView& b, const StepWs& w) {
+// the edge rows here, the negatives' rows by k_prep's generic blocks
+int launch_rescal_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
+                       const BatchView& b, const StepWs& w) {
   size_t smem = 4 * (size_t)p.D * sizeof(float);
   KGE_LAUNCH(c, k_rescal_fwd, (unsigned)p.B, kBlock, smem, p, nullptr, nullptr, nullptr, ent, rel, b, w, false, true, true);
   return launch_prep_nonedge(c, p, ent, rel, b, w);

@@ -276,21 +276,14 @@ __global__ void __launch_bounds__(kRowBlock, 3) k_prep(StepParams p, TableView e
   }
 }
 
-// dynamic shared memory of a k_prep launch (*bytes): the staging buffer exists only where the transposed slabs do; beyond
-// 48 KB (d > 356) the kernel has to opt in.  An error here means the launch must not be made.
-template <int MODEL, int KIT>
-cudaError_t prep_optin(const StepWs& w, int D, size_t* bytes) {
-  *bytes = (w.AhiT || w.BhiT) ? prep_stage_bytes(D) : 0;
-  if (*bytes > kSmemOptinMax) return cudaErrorInvalidValue;      // umma_supported keeps such rows off the wgmma engine
-  static size_t optin[64] = {};          // the opt-in shared-memory size is a per-device function attribute
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (*bytes > 48 * 1024 && dev >= 0 && dev < 64 && *bytes > optin[dev]) {
-    const cudaError_t e = cudaFuncSetAttribute(k_prep<MODEL, KIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*bytes);
-    if (e != cudaSuccess) return e;
-    optin[dev] = *bytes;
-  }
-  return cudaSuccess;
+// dynamic shared memory of a k_prep launch: the staging buffer exists only where the transposed slabs do (beyond 48 KB,
+// d > 356, the kernel has to opt in)
+size_t prep_smem(const StepWs& w, int D) { return (w.AhiT || w.BhiT) ? prep_stage_bytes(D) : 0; }
+
+// k_prep's launch error (with whatever an earlier launch of the step left behind)
+int prep_launched(int D) {
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? KGE_OK : fail(KGE_ERR_CUDA, "k_prep launch (d=%d): %s", D, cudaGetErrorString(e));
 }
 
 // ExternalEmbedding.__call__ on pos_g.ndata['id'] (general_models.py:548): NC[u,:] = ent[node_ids[u],:], one warp per
@@ -382,33 +375,31 @@ __global__ void __launch_bounds__(kRowBlock) k_prep_dense(StepParams p, const fl
     default: break;                                                         \
   }
 
-cudaError_t launch_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
-                        const BatchView& b, const StepWs& w) {
+int launch_prep(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
+                const BatchView& b, const StepWs& w) {
   const int rows = prep_block_rows(w);
   const int blocks = p.C * (ceil_div(p.Cs, rows) + ceil_div(p.Ns, rows));
-  size_t smem = 0;
-  cudaError_t e = cudaSuccess;
+  const size_t smem = prep_smem(w, p.D);
+  int rc = KGE_OK;
   // sharded tables: deeper per-lane load batches hide the NVLink latency; local HBM prefers occupancy
   if (ent.n_shards > 1) {
-    KGE_DISPATCH_MODEL(p.model, if ((e = prep_optin<M, 4>(w, p.D, &smem)) == cudaSuccess)
+    KGE_DISPATCH_MODEL(p.model, if (!(rc = smem_optin((const void*)k_prep<M, 4>, smem)))
                                   KGE_LAUNCH(c, (k_prep<M, 4>), blocks, kRowBlock, smem, p, ent, rel, b, w, 0));
   } else {
-    KGE_DISPATCH_MODEL(p.model, if ((e = prep_optin<M, 1>(w, p.D, &smem)) == cudaSuccess)
+    KGE_DISPATCH_MODEL(p.model, if (!(rc = smem_optin((const void*)k_prep<M, 1>, smem)))
                                   KGE_LAUNCH(c, (k_prep<M, 1>), blocks, kRowBlock, smem, p, ent, rel, b, w, 0));
   }
-  return e != cudaSuccess ? e : cudaGetLastError();
+  return rc ? rc : prep_launched(p.D);
 }
 
-// the negatives' blocks only (RESCAL runs its own per-edge kernel)
-cudaError_t launch_prep_nonedge(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
-                                const BatchView& b, const StepWs& w) {
-  size_t smem = 0;
-  const cudaError_t e = prep_optin<KGE_DISTMULT, 1>(w, p.D, &smem);
-  if (e != cudaSuccess) return e;
+int launch_prep_nonedge(const LaunchCtx& c, const StepParams& p, const TableView& ent, const TableView& rel,
+                        const BatchView& b, const StepWs& w) {
+  const size_t smem = prep_smem(w, p.D);
+  if (int rc = smem_optin((const void*)k_prep<KGE_DISTMULT, 1>, smem)) return rc;
   const int rows = prep_block_rows(w);
   KGE_LAUNCH(c, (k_prep<KGE_DISTMULT, 1>), p.C * ceil_div(p.Ns, rows), kRowBlock, smem, p, ent, rel, b, w,
              p.C * ceil_div(p.Cs, rows));
-  return cudaGetLastError();
+  return prep_launched(p.D);
 }
 
 void launch_prep_dense(const LaunchCtx& c, const StepParams& p, const float* head, const float* relr,
@@ -1158,7 +1149,8 @@ int launch_update(const LaunchCtx& c, const StepParams& p, const TableView& ent,
     if (c.launch_counter) ++*c.launch_counter;
     if (e == cudaSuccess) return KGE_OK;
     cudaGetLastError();
-    return KGE_ERR_CUDA;
+    return fail(KGE_ERR_CUDA, "cooperative launch of k_update failed: %s (set KGE_B200_NO_COOP=1 for the three-launch form)",
+                cudaGetErrorString(e));
   }
   for (int ph = 1; ph <= 3; ++ph) {
     a.phase_lo = a.phase_hi = ph;

@@ -151,7 +151,7 @@ __device__ __forceinline__ float sqrta(float x) { float y; asm("sqrt.approx.ftz.
 }  // namespace tc
 
 // host side (kge_umma.cu): cached cuTensorMapEncodeTiled of a 2-D fp32 matrix [rows, cols] with box {32 cols, box_rows},
-// 128-byte swizzle, zero OOB fill.
-bool tc_make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen);
+// 128-byte swizzle, zero OOB fill.  KGE_OK, or KGE_ERR_CUDA with the message set.
+int tc_make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows);
 
 }  // namespace kge

@@ -207,10 +207,23 @@ struct MapCache {
 };
 thread_local MapCache g_maps;
 
-bool make_map_uncached(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err,
-                       size_t errlen);
+template <int MODE>
+int launch_gemm(const LaunchCtx& c, const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
+                const CUtensorMap& bl, const GemmArgs& g) {
+  const size_t smem = (size_t)kStages * kStageBytes + 1024;
+  if (int rc = smem_optin((const void*)k_wgmma_gemm<MODE>, smem)) return rc;
+  dim3 grid((g.N + kTileN - 1) / kTileN, (g.M + kTileM - 1) / kTileM, g.C);
+  const char* nm = MODE == G_SCORE ? "k_wgmma_gemm<score S=A.Bn^T>"
+                                   : (MODE == G_GA ? "k_wgmma_gemm<grad_a GA=V.Bn>" : "k_wgmma_gemm<grad_b GB=V^T.A>");
+  KGE_LAUNCH_NAMED(c, nm, (k_wgmma_gemm<MODE>), grid, kThreads, smem, ah, al, bh, bl, g);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(KGE_ERR_CUDA, "wgmma gemm launch: %s", cudaGetErrorString(e));
+  return KGE_OK;
+}
 
-bool make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen) {
+}  // namespace
+
+int tc_make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows) {
   MapCache& mc = g_maps;
   int dev = 0;
   cudaGetDevice(&dev);
@@ -218,21 +231,11 @@ bool make_map(CUtensorMap* m, const float* base, long long rows, long long cols,
     const MapKey& k = mc.keys[i];
     if (k.base == base && k.rows == rows && k.cols == cols && k.box_rows == box_rows && k.dev == dev) {
       *m = mc.maps[i];
-      return true;
+      return KGE_OK;
     }
   }
-  if (!make_map_uncached(m, base, rows, cols, box_rows, err, errlen)) return false;
-  int slot = mc.n < MapCache::kN ? mc.n++ : (mc.next++ % MapCache::kN);
-  mc.keys[slot] = MapKey{base, rows, cols, box_rows, dev};
-  mc.maps[slot] = *m;
-  return true;
-}
-
-// 2-D fp32 row-major matrix [rows, cols], box {32 cols, box_rows}, 128-byte swizzle, zero OOB fill
-bool make_map_uncached(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err,
-                       size_t errlen) {
   encode_fn_t enc = get_encode();
-  if (!enc) { snprintf(err, errlen, "cuTensorMapEncodeTiled not available"); return false; }
+  if (!enc) return fail(KGE_ERR_CUDA, "cuTensorMapEncodeTiled not available");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)cols * 4};
   cuuint32_t box[2] = {32u, (cuuint32_t)box_rows};
@@ -241,35 +244,12 @@ bool make_map_uncached(CUtensorMap* m, const float* base, long long rows, long l
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { snprintf(err, errlen, "cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld box_rows=%d", (int)r, rows, cols, box_rows); return false; }
-  return true;
-}
-
-template <int MODE>
-int launch_gemm(const LaunchCtx& c, const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh,
-                const CUtensorMap& bl, const GemmArgs& g, char* err, size_t errlen) {
-  const size_t smem = (size_t)kStages * kStageBytes + 1024;
-  static bool attr_set[64] = {};          // the opt-in shared-memory size is a per-device function attribute
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_wgmma_gemm<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { snprintf(err, errlen, "cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return KGE_ERR_CUDA; }
-    attr_set[dev] = true;
-  }
-  dim3 grid((g.N + kTileN - 1) / kTileN, (g.M + kTileM - 1) / kTileM, g.C);
-  const char* nm = MODE == G_SCORE ? "k_wgmma_gemm<score S=A.Bn^T>"
-                                   : (MODE == G_GA ? "k_wgmma_gemm<grad_a GA=V.Bn>" : "k_wgmma_gemm<grad_b GB=V^T.A>");
-  KGE_LAUNCH_NAMED(c, nm, (k_wgmma_gemm<MODE>), grid, kThreads, smem, ah, al, bh, bl, g);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { snprintf(err, errlen, "wgmma gemm launch: %s", cudaGetErrorString(e)); return KGE_ERR_CUDA; }
+  if (r != CUDA_SUCCESS)
+    return fail(KGE_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld box_rows=%d", (int)r, rows, cols, box_rows);
+  int slot = mc.n < MapCache::kN ? mc.n++ : (mc.next++ % MapCache::kN);
+  mc.keys[slot] = MapKey{base, rows, cols, box_rows, dev};
+  mc.maps[slot] = *m;
   return KGE_OK;
-}
-
-}  // namespace
-
-bool tc_make_map(CUtensorMap* m, const float* base, long long rows, long long cols, int box_rows, char* err, size_t errlen) {
-  return make_map(m, base, rows, cols, box_rows, err, errlen);
 }
 
 bool umma_supported(const StepParams& p) {
@@ -288,43 +268,43 @@ GemmArgs base_args(const StepParams& p) {
 }  // namespace
 
 // S = A . Bn^T  (+ TransE_l2 distance epilogue)
-int umma_score(const LaunchCtx& c, const StepParams& p, const StepWs& w, char* err, size_t errlen) {
+int umma_score(const LaunchCtx& c, const StepParams& p, const StepWs& w) {
   // operands arrive already split: k_prep writes A / Bn as TF32 hi/lo, k_loss writes V hi/lo
   CUtensorMap ah, al, bh, bl;
   const long long rowsA = p.B * (long long)slab_blocks(p.D), rowsB = p.Nn * (long long)slab_blocks(p.D);
-  if (!make_map(&ah, w.Ahi, rowsA, 32, kTileM, err, errlen) || !make_map(&al, w.Alo, rowsA, 32, kTileM, err, errlen) ||
-      !make_map(&bh, w.Bhi, rowsB, 32, kTileN, err, errlen) || !make_map(&bl, w.Blo, rowsB, 32, kTileN, err, errlen))
+  if (tc_make_map(&ah, w.Ahi, rowsA, 32, kTileM) || tc_make_map(&al, w.Alo, rowsA, 32, kTileM) ||
+      tc_make_map(&bh, w.Bhi, rowsB, 32, kTileN) || tc_make_map(&bl, w.Blo, rowsB, 32, kTileN))
     return KGE_ERR_CUDA;
   GemmArgs g = base_args(p);
   g.mode = G_SCORE; g.M = p.Cs; g.N = p.Ns; g.K = p.D;
   g.a_nblk = slab_blocks(p.D); g.a_R = p.Cs; g.b_nblk = slab_blocks(p.D); g.b_R = p.Ns;
   g.out = w.S; g.out2 = w.V; g.a2 = w.a2; g.b2 = w.b2;
-  return launch_gemm<G_SCORE>(c, ah, al, bh, bl, g, err, errlen);
+  return launch_gemm<G_SCORE>(c, ah, al, bh, bl, g);
 }
 
 // side_b == false: GA = V . Bn ; side_b == true: G_neg = V^T . A (+ epilogue), in place over Bn
-int umma_grad(const LaunchCtx& c, const StepParams& p, const StepWs& w, bool side_b, char* err, size_t errlen) {
+int umma_grad(const LaunchCtx& c, const StepParams& p, const StepWs& w, bool side_b) {
   CUtensorMap ah, al, bh, bl;
   GemmArgs g = base_args(p);
   g.colsum = w.colsum;
   if (!side_b) {
     // A operand: V slabs [C][Ns/32][Cs][32]; B operand: Bn^T slabs [C][Ns/32][D][32]; K = j
     const long long rowsV = p.B * (long long)slab_blocks(p.Ns), rowsB = (long long)p.C * slab_blocks(p.Ns) * p.D;
-    if (!make_map(&ah, w.Vhi, rowsV, 32, kTileM, err, errlen) || !make_map(&al, w.Vlo, rowsV, 32, kTileM, err, errlen) ||
-        !make_map(&bh, w.BhiT, rowsB, 32, kTileN, err, errlen) || !make_map(&bl, w.BloT, rowsB, 32, kTileN, err, errlen))
+    if (tc_make_map(&ah, w.Vhi, rowsV, 32, kTileM) || tc_make_map(&al, w.Vlo, rowsV, 32, kTileM) ||
+        tc_make_map(&bh, w.BhiT, rowsB, 32, kTileN) || tc_make_map(&bl, w.BloT, rowsB, 32, kTileN))
       return KGE_ERR_CUDA;
     g.a_nblk = slab_blocks(p.Ns); g.a_R = p.Cs; g.b_nblk = slab_blocks(p.Ns); g.b_R = p.D;
     g.mode = G_GA; g.M = p.Cs; g.N = p.D; g.K = p.Ns; g.out = w.GA;
-    return launch_gemm<G_GA>(c, ah, al, bh, bl, g, err, errlen);
+    return launch_gemm<G_GA>(c, ah, al, bh, bl, g);
   }
   // A operand: V^T slabs [C][Cs/32][Ns][32]; B operand: A^T slabs [C][Cs/32][D][32]; K = i
   const long long rowsV = (long long)p.C * slab_blocks(p.Cs) * p.Ns, rowsA = (long long)p.C * slab_blocks(p.Cs) * p.D;
-  if (!make_map(&ah, w.VhiT, rowsV, 32, kTileM, err, errlen) || !make_map(&al, w.VloT, rowsV, 32, kTileM, err, errlen) ||
-      !make_map(&bh, w.AhiT, rowsA, 32, kTileN, err, errlen) || !make_map(&bl, w.AloT, rowsA, 32, kTileN, err, errlen))
+  if (tc_make_map(&ah, w.VhiT, rowsV, 32, kTileM) || tc_make_map(&al, w.VloT, rowsV, 32, kTileM) ||
+      tc_make_map(&bh, w.AhiT, rowsA, 32, kTileN) || tc_make_map(&bl, w.AloT, rowsA, 32, kTileN))
     return KGE_ERR_CUDA;
   g.a_nblk = slab_blocks(p.Cs); g.a_R = p.Ns; g.b_nblk = slab_blocks(p.Cs); g.b_R = p.D;
   g.mode = G_GB; g.M = p.Ns; g.N = p.D; g.K = p.Cs; g.out = w.Bn;
-  return launch_gemm<G_GB>(c, ah, al, bh, bl, g, err, errlen);
+  return launch_gemm<G_GB>(c, ah, al, bh, bl, g);
 }
 
 }  // namespace kge
