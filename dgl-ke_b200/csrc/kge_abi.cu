@@ -678,6 +678,9 @@ static int forward_backward_impl(kge_handle_t h, const kge_step_cfg_t* cfg, cons
   }
   if (p.model == KGE_RESCAL) launch_rescal_chain(c, p, ve, vr, b, w);
   else launch_chain(c, p, ve, vr, b, w);
+  // deferred relations into the caller's buffers: a chain that left per-edge rows (RESCAL) has them summed here, so
+  // that the begin call fills the buffers for every model
+  if (fused_step && p.rel_deferred && !p.rel_dense && h->ext_rg) launch_rel_grad_dense(c, p, b, w, h->ext_rg, h->ext_rgs);
   // 3-call API: the log scalars are due now; fused step: the update kernel reduces them (it also produces the unique
   // nodes' share of the regulariser when NC is skipped)
   if (!fused_step) launch_reduce_log(c, p, b.edge_weight, w, logdst, true);

@@ -196,21 +196,26 @@ def main(argv=None):
     return model
 
 
+def hyper_from_args(args):
+    """The step hyper-parameters of the parsed command line: every field of engine.Hyper, the loss flags included."""
+    from .engine import Hyper
+    return Hyper(model=args.model_name, hidden_dim=args.hidden_dim, gamma=args.gamma, lr=args.lr,
+                 reg_coef=args.regularization_coef, reg_norm=args.regularization_norm,
+                 adversarial=args.neg_adversarial_sampling, adv_temperature=args.adversarial_temperature,
+                 double_ent=args.double_ent, double_rel=args.double_rel, loss_genre=args.loss_genre,
+                 margin=args.margin, pairwise=args.pairwise, neg_deg_sample=args.neg_deg_sample)
+
+
 def _multi_gpu_worker(rank, world, args, n_ent, n_rel, edges, port):
     """One process per GPU (reference: train.py:298-317 forks one process per GPU over a shared host table)."""
     import torch.distributed as dist
     from .dist import ShardedTrainer
-    from .engine import Hyper
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
                       LOCAL_RANK=str(rank))
     dev = th.device("cuda", args.gpu[rank])
     th.cuda.set_device(dev)
     dist.init_process_group("nccl", device_id=dev)
-    hp = Hyper(model=args.model_name, hidden_dim=args.hidden_dim, gamma=args.gamma, lr=args.lr,
-               reg_coef=args.regularization_coef, reg_norm=args.regularization_norm,
-               adversarial=args.neg_adversarial_sampling, adv_temperature=args.adversarial_temperature,
-               double_ent=args.double_ent, double_rel=args.double_rel)
-    trainer = ShardedTrainer(hp, n_ent, n_rel, dev, seed=0)
+    trainer = ShardedTrainer(hyper_from_args(args), n_ent, n_rel, dev, seed=0)
     # edge partition: the edges whose head row this rank owns (half of the positive-node traffic stays on the GPU);
     # KGE_B200_EDGE_PART=random gives the reference's RandomPartition (dataloader/sampler.py:256-290)
     if os.environ.get("KGE_B200_EDGE_PART", "head_owner") == "random":
@@ -261,6 +266,8 @@ def train_multi_gpu(args, n_ent, n_rel, edges):
     world = len(args.gpu)
     if args.has_edge_importance:
         raise SystemExit("--has_edge_importance is single-GPU only here")
+    if args.neg_deg_sample:
+        raise SystemExit("--neg_deg_sample is single-GPU only here: it needs an unsharded entity table")
     port = 29400 + os.getpid() % 1000
     edges = tuple(np.ascontiguousarray(e, dtype=np.int64) for e in edges)
     mp.spawn(_multi_gpu_worker, args=(world, args, n_ent, n_rel, edges, port), nprocs=world, join=True)

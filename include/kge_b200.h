@@ -283,8 +283,9 @@ KGE_API int kge_debug_set_dump(kge_handle_t h, float* coef_dump);
  * Adagrad update on every replica and zeroes the buffers. */
 KGE_API int kge_set_relation_mode(kge_handle_t h, int deferred);
 /* Deferred mode, fused step: caller-owned dense buffers rg [num_rel, D_r] and rgs [num_rel] (zero between steps) that
- * kge_step_fused_begin sums the per-relation gradients / mean squares into directly (no per-edge rows, no
- * kge_rel_grad_dense); the caller all-reduces them and calls kge_rel_apply_dense.  NULL, NULL = off. */
+ * kge_step_fused_begin sums the per-relation gradients / mean squares into (no kge_rel_grad_dense; RESCAL, whose
+ * chain kernel writes per-edge rows, gets one extra summing launch); the caller all-reduces them and calls
+ * kge_rel_apply_dense.  NULL, NULL = off. */
 KGE_API int kge_set_relation_buffers(kge_handle_t h, float* rg, float* rgs);
 KGE_API int kge_rel_grad_dense(kge_handle_t h, float* rg, float* rgs, void* stream);
 KGE_API int kge_rel_apply_dense(kge_handle_t h, const kge_table_t* rel, float* rg, float* rgs, float lr, void* stream);

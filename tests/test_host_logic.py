@@ -46,6 +46,33 @@ def test_defaults_worth_knowing():
     assert (a.regularization_coef, a.regularization_norm, a.loss_genre, a.gpu) == (2e-6, 3, "Logsigmoid", [-1])
 
 
+def test_multi_gpu_hyper_carries_every_parsed_field():
+    """The multi-GPU worker builds its step configuration with train.hyper_from_args: every field of engine.Hyper comes
+    from its flag, set here to a value other than the default, so a dropped flag shows up as the default."""
+    import dataclasses
+    from dglke_b200.engine import Hyper
+    from dglke_b200.train import hyper_from_args
+    argv = {"model": (["--model_name", "RotatE"], "RotatE"), "hidden_dim": (["--hidden_dim", "72"], 72),
+            "gamma": (["--gamma", "7.5"], 7.5), "lr": (["--lr", "0.3"], 0.3),
+            "reg_coef": (["--regularization_coef", "3e-5"], 3e-5), "reg_norm": (["--regularization_norm", "2"], 2),
+            "adversarial": (["-adv"], True), "adv_temperature": (["-a", "0.4"], 0.4),
+            "double_ent": (["-de"], True), "double_rel": (["-dr"], True), "loss_genre": (["--loss_genre", "Hinge"], "Hinge"),
+            "margin": (["-m", "2.5"], 2.5), "pairwise": (["-pw"], True), "neg_deg_sample": (["--neg_deg_sample"], True)}
+    fields = {f.name: f.default for f in dataclasses.fields(Hyper)}
+    assert sorted(argv) == sorted(fields), "a Hyper field without a flag here: extend this test and hyper_from_args"
+    hp = hyper_from_args(utils.ArgParser().parse_args(sum((a for a, _ in argv.values()), [])))
+    for name, (_, want) in argv.items():
+        assert want != fields[name], name
+        assert getattr(hp, name) == want, name
+
+
+def test_multi_gpu_refuses_neg_deg_sample():
+    from dglke_b200.train import train_multi_gpu
+    args = utils.ArgParser().parse_args(["--gpu", "0", "1", "--neg_deg_sample"])
+    with pytest.raises(SystemExit, match="neg_deg_sample"):
+        train_multi_gpu(args, 100, 4, (np.zeros(8), np.zeros(8), np.zeros(8)))
+
+
 def test_batch_size_rounding():
     assert utils.get_compatible_batch_size(1000, 256) == 1024     # utils.py:27-33
     assert utils.get_compatible_batch_size(1024, 256) == 1024
