@@ -317,12 +317,12 @@ int carve(kge_context* h, const StepParams& p, StepWs* w, cudaStream_t stream, c
       {&w->S, BNs, !fused || opt.want_scores}, {&w->V, BNs, !fused},
       {&w->pos, B, true}, {&w->gpos, B, true}, {&w->pnorm, B, true}, {&w->a2, B, true}, {&w->b2, Nn, true},
       {&w->rowsum, B, true}, {&w->colsum, Nn, true}, {&w->pl, B, true}, {&w->nl, B, true}, {&w->wbar, 4, true},
-      {&w->gsr, B, true}, {&w->gsn, Nn, true}, {&w->stat_m, B, true}, {&w->stat_k, B, true},
+      {&w->gsr, B, true}, {&w->gsn, Nn, true}, {&w->colpart, (size_t)ceil_div(p.Cs, 128) * Nn, fused},
       {&w->Mt, BD, p.model == KGE_RESCAL},
       {&w->Ahi, sA, um}, {&w->Alo, sA, um}, {&w->Bhi, sB, um}, {&w->Blo, sB, um},
       {&w->Vhi, sV, um && !fused}, {&w->Vlo, sV, um && !fused},
       {&w->AhiT, sAT, um}, {&w->AloT, sAT, um}, {&w->BhiT, sBT, um}, {&w->BloT, sBT, um},
-      {&w->VhiT, sVT, um && !fused}, {&w->VloT, sVT, um && !fused},
+      {&w->VhiT, sVT, um}, {&w->VloT, sVT, um},
       // U-dependent tail
       {&w->NC, U * p.D, p.use_nc != 0},
       {&w->regp, B + Nn + (U ? 2 * B : 0), true},

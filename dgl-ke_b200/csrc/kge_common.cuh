@@ -88,8 +88,7 @@ struct StepWs {
   float* wbar;     // [1]      mean edge weight
   float* gsr;      // [B]      mean(GR_i^2) per edge (relation Adagrad phase 1)
   float* gsn;      // [Nn]     mean(G_neg_j^2) per negative row (fused kernel, mode N)
-  float* stat_m;   // [B]      softmax shift of row i, log2 domain (fused kernel: mode P -> mode N)
-  float* stat_k;   // [B]      w_i / (2B den_i)                    (fused kernel: mode P -> mode N)
+  float* colpart;  // [ceil(Cs/128)][Nn] sum_i V_ij over each 128-row tile of positives (fused kernel: mode P -> mode N)
   float* rg;       // [n_rel, Dr] dense per-relation gradient sums (rel_dense), zero between steps
   float* rgs;      // [n_rel]     dense per-relation sums of mean(g^2)          , zero between steps
   const float* BnRaw;         // [Nn, D] negative rows staged by the previous step's prefetch warps, or null
@@ -105,7 +104,7 @@ struct StepWs {
   // contract over the rows of these matrices
   float *AhiT, *AloT; // [C][Cs/32][D][32]
   float *BhiT, *BloT; // [C][Ns/32][D][32]
-  float *VhiT, *VloT; // [C][Cs/32][Ns][32]
+  float *VhiT, *VloT; // [C][Cs/32][Ns][32]   (fused step: written by mode P, the A operand of mode N)
 };
 
 struct BatchView {

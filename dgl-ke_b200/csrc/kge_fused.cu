@@ -1,30 +1,30 @@
-// kge_fused.cu -- the fused contraction kernel of the step (wgmma / TMA / mbarrier, sm_90a):
+// kge_fused.cu -- the two contraction kernels of the fused step (wgmma / TMA / mbarrier, sm_90a):
 //
-//   S = X . Y^T  (tensor cores, accumulator in registers)  ->  loss / self-adversarial softmax / backward
-//   coefficients V computed in place in the accumulator registers  ->  G = V . Y  (tensor cores, V as the REGISTER
-//   A operand of wgmma, split into TF32 hi/lo per k-step)  ->  epilogue.
+//   k_fused<P>  rows = positives i, columns = negatives j:
+//               S = A.Bn^T (tensor cores, accumulator in registers) -> loss / self-adversarial softmax / backward
+//               coefficients V computed in place in the accumulator registers -> GA = V.Bn (tensor cores, V as the
+//               REGISTER A operand of wgmma, split into TF32 hi/lo per k-step) -> epilogue.
+//               Replaces create_neg (score_fun.py:91-108,268-286,345-376,427-449), LossGenerator.get_total_loss
+//               (loss.py:69-98) and the dL/da half of loss.backward().  The score matrix S never leaves the SM; V leaves
+//               it once, as the transposed TF32 hi/lo slabs V^T[c][i / 32][j][i % 32] plus per-tile column sums
+//               sum_i V_ij, for k_fused<N>.
+//   k_fused<N>  rows = negatives j:  G_neg = V^T.A - colsum*b + reg'(b), mean(G_neg^2)  (the dL/db half of
+//               loss.backward() plus phase 1 of ExternalEmbedding.update for the negatives, tensor_models.py:316-328).
+//               One pipelined GEMM over K = Cs with both operands from shared memory: V^T slabs (written by k_fused<P>)
+//               and the transposed A slabs (written by k_prep).
 //
-// The negative-score matrix S and the coefficient matrix V never leave the SM.  The kernel runs twice per step:
+// Handing V over costs 2 x 4 B x C x Cs x Ns of HBM traffic each way (23.6 MB at 66 chunks of 200 x 200); recomputing
+// it in the second orientation cost a whole K = D GEMM per chunk plus the loss epilogue, and an S accumulator that
+// crowded the register file.  fp32 fidelity: operands are TF32 hi/lo pairs and every k-step issues hi*hi + hi*lo +
+// lo*hi (3xTF32, fp32 accumulation).  wgmma reads TF32 operands K-major only: GEMMs that contract over the rows of a
+// matrix take its transposed slabs (kge_common.cuh:slabT_off).
 //
-//   mode P  rows = positives i, columns = negatives j:   S = A.Bn^T, row softmax, GA = V.Bn
-//           replaces create_neg (score_fun.py:91-108,268-286,345-376,427-449), LossGenerator.get_total_loss
-//           (loss.py:69-98) and the dL/da half of loss.backward()
-//   mode N  rows = negatives j, columns = positives i:   S^T = Bn.A^T, V^T from the row statistics mode P left
-//           behind, G_neg = V^T.A - colsum*b + reg'(b), mean(G_neg^2)  (the dL/db half of loss.backward() plus
-//           phase 1 of ExternalEmbedding.update for the negatives, tensor_models.py:316-328)
-//
-// Recomputing S in the second orientation costs one extra tensor-core GEMM per chunk and removes every HBM/L2 round
-// trip of S and V (and the k_loss / k_colsum / k_state_add launches).  fp32 fidelity: operands are TF32 hi/lo pairs
-// and every k-step issues hi*hi + hi*lo + lo*hi (3xTF32, fp32 accumulation).
-//
-// wgmma reads TF32 operands K-major only: GEMM1 takes the slabs of X and Y, GEMM2 the TRANSPOSED slabs of Y that
-// k_prep writes next to them (kge_common.cuh:slabT_off).
-//
-// CTA = 384 threads: warpgroups 0 and 1 (warps 0-7) each own 64 rows of the 128-row tile -- MMA issue, softmax and
-// epilogue all on the accumulator fragment, a row lives in the 4 lanes of a quad; warp 8 TMA producer, warp 9 idle (setmaxnreg acts on whole warpgroups),
-// warps 10-11 prefetch the next step's rows.  Persistent over (chunk, 128-row tile) work items.  Shared memory: one
-// 192 KB ring used as nS1 stages {X_hi,X_lo,Y_hi,Y_lo} by GEMM1 and as nS2 stages {Y^T_hi,Y^T_lo} by GEMM2, whose
-// output is produced in 128-column chunks.
+// CTA = 384 threads: warpgroups 0 and 1 (warps 0-7) each own 64 rows of the 128-row tile -- MMA issue and epilogue on
+// the accumulator fragment, a row lives in the 4 lanes of a quad; warp 8 TMA producer, warp 9 idle (setmaxnreg acts on
+// whole warpgroups), warps 10-11 prefetch the next step's rows.  Persistent over (chunk, 128-row tile) work items.
+// Shared memory: one 192 KB ring.  k_fused<P> uses it as nS1 stages {X_hi,X_lo,Y_hi,Y_lo} for GEMM1 and as nS2 stages
+// {Y^T_hi,Y^T_lo} for GEMM2, whose output is produced in 128-column chunks; k_fused<N> as nS stages
+// {V^T_hi,V^T_lo,A^T_hi,A^T_lo} of one output-column chunk of width NW.
 #include <cuda.h>
 #include <cstdio>
 #include <cstdlib>
@@ -43,40 +43,39 @@ constexpr int kProducerWarp = 8;
 constexpr int kMaxS1 = 4, kMaxS2 = 8;
 constexpr int kMaxPf = 8;                          // row slots per prefetch warp
 constexpr uint32_t kRingBytes = 192 * 1024;
-constexpr int kWc = 128;                           // GEMM2 output-column chunk = wgmma N
+constexpr int kWc = 128;                           // k_fused<P> GEMM2 output-column chunk = wgmma N
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
-
-enum { F_P = 0, F_N = 1 };
 
 struct FusedArgs {
   int model, adversarial;
   float gamma, Tl2e, inv2B, uni;
   float reg_coef;
   int reg_norm;
-  int C, Rx, Ry, D;      // rows per chunk on the lane side / on the column side, row length
-  int N1;                // wgmma N of GEMM1: the kernel variant's width, >= Ry
+  int C, Rx, Ry, D;      // rows per chunk on the lane side / on the contraction side of the last GEMM, row length
+  int N1;                // P: wgmma N of GEMM1 (the kernel variant's width, >= Ry);  N: output-column chunk width
   int nblkD;             // 32-column slab blocks of D
-  int nS1, nS2;
+  int nS1, nS2;          // P: GEMM1 / GEMM2 stages;  N: nS1 stages
   uint32_t stage1Bytes, stage2Bytes;
-  const float* x2;       // |x|^2 per lane-side row   (TransE_l2)
-  const float* y2;       // |y|^2 per column-side row (TransE_l2)
+  float *VhiT, *VloT;    // [C][Cs/32][Ns][32] coefficients V_ij as TF32 hi/lo (P writes, N reads)
+  float* colpart;        // [ceil(Cs/128)][C*Ns] per-tile column sums sum_i V_ij (TransE_l2; P writes, N reads)
+  int ncolpart;          // N: number of those partials
   // mode P
+  const float* x2;       // |a|^2 per positive (TransE_l2)
+  const float* y2;       // |b|^2 per negative (TransE_l2)
   const float* pos;      // [B] positive scores
   const float* wt;       // [B] edge weights or null
   const float* wbar;     // [1] mean edge weight (with wt)
-  float *gpos, *rowsum, *pl, *nl, *stat_m, *stat_k;
+  float *gpos, *rowsum, *pl, *nl;
   float* dumpS;          // optional [C*Rx, Ry]: negative scores (kge_debug_read)
-  float* dumpV;          // optional [C*Rx, Ry]: backward coefficients (tests)
+  float* dumpV;          // optional: P [C*Cs, Ns] and N [C*Ns, Cs] views of the backward coefficients (tests)
   // mode N
-  const float* cstat_m;  // per positive: softmax shift (log2 domain)
-  const float* cstat_k;  // per positive: w_i / (2B den_i)  (or w_i / (2B Ns))
-  const float *Xhi, *Xlo;  // slabs of the lane-side rows (negatives): b = hi + lo in the epilogue
-  const long long* xids;   // mode N, one GPU: entity ids of the lane-side rows -- b is then read from the table itself
+  const float *Xhi, *Xlo;  // slabs of the negatives' rows: b = hi + lo in the epilogue
+  const long long* xids;   // mode N, one GPU: entity ids of the negatives -- b is then read from the table itself
   TableView xtab;          //   (one fp32 load instead of hi + lo; nothing updates the table before k_update)
-  const float* xraw;       // mode N, sharded + staged: the lane-side rows as fp32 [C*Rx, D] (the previous step's prefetch)
-  float* gsn;            // [C*Rx] mean(G_neg^2)
-  float* out;            // P: GA [C*Rx, D]; N: G_neg [C*Rx, D]
+  const float* xraw;       // mode N, sharded + staged: the negatives' rows as fp32 [C*Ns, D] (the previous step's prefetch)
+  float* gsn;            // [C*Ns] mean(G_neg^2)
+  float* out;            // P: GA [C*Cs, D]; N: G_neg [C*Ns, D]
   // next step's rows, copied by the two spare warps while this step's tiles are computed (sharded tables: the remote-row
   // latency of step k+1 hides behind the tensor-core work of step k).  Virtual row v of [nodes | negatives]; this launch
   // takes the v with v % 2 == pf_parity (the P and the N kernel split the list).
@@ -102,15 +101,75 @@ __device__ __forceinline__ float reg_grad_fast(float b, int norm, float coef) {
 
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-template <int MODE, int NV>
+// ================================ prefetch warps 10, 11 (both kernels) ================================
+// Each warp streams table rows (peer memory when the table is sharded) through a few shared-memory slots into the
+// next step's buffers: bulk load -> mbarrier -> bulk store, S slots per warp re-used round robin.  The loop is warp-uniform
+// (one elected lane issues): the row ids arrive 32 at a time, one coalesced load per lane, and are handed out by shuffle
+// -- a per-row dependent id load by a single lane costs more than the copy itself.
+__device__ __forceinline__ void prefetch_rows(const FusedArgs& g, uint8_t* ring, uint64_t (*pf_full)[kMaxPf], int w, int lane) {
+  const int S = g.pf_slots;
+  const long long nU = g.pf_nU_dev ? *g.pf_nU_dev : g.pf_nU;
+  const long long total = nU + g.pf_nNeg;
+  const long long nhalf = total > g.pf_parity ? (total - g.pf_parity + 1) / 2 : 0;   // v = parity + 2 j < total
+  const long long stride = 2ll * gridDim.x, j0 = 2ll * blockIdx.x + w;
+  const long long n = j0 < nhalf ? (nhalf - j0 + stride - 1) / stride : 0;
+  uint8_t* slots = ring + g.pf_off + (size_t)w * S * g.pf_row_bytes;
+  auto vrow = [&](long long k) { return g.pf_parity + 2 * (j0 + k * stride); };
+  auto fetch_ids = [&](long long kb) {            // ids of items kb .. kb+31, one per lane
+    const long long k = kb + lane;
+    if (k >= n) return 0ll;
+    const long long v = vrow(k);
+    return v < nU ? g.pf_node_ids[v] : g.pf_neg_ids[v - nU];
+  };
+  long long ids_lo = fetch_ids(0), ids_hi = fetch_ids(32);      // items [base, base+32) and [base+32, base+64)
+  long long base = 0;
+  auto load = [&](long long k) {                  // k in [base, base + 64)
+    const int o = (int)(k - base);
+    const long long id = __shfl_sync(0xffffffffu, o < 32 ? ids_lo : ids_hi, o & 31);
+    const int s = (int)(k % S);
+    if (elect_one()) {
+      mbar_expect_tx(&pf_full[w][s], g.pf_row_bytes);
+      bulk_g2s(slots + (size_t)s * g.pf_row_bytes, row_ptr(g.xtab, id), g.pf_row_bytes, &pf_full[w][s]);
+    }
+    __syncwarp();
+  };
+  for (long long k = 0; k < n && k < S; ++k) load(k);
+  // A slot is re-loaded L stores after its own store was issued (S - L loads in flight).  L = 1 keeps the most loads in
+  // flight, which is what matters when the rows are remote; a larger L (KGE_B200_PF_LAG) never waits on the copy
+  // engine's queue for the newest store.
+  const int L = g.pf_lag < S - 1 ? g.pf_lag : (S > 2 ? S - 2 : 1);
+  for (long long k = 0; k < n; ++k) {
+    const int s = (int)(k % S);
+    mbar_wait(&pf_full[w][s], (uint32_t)((k / S) & 1));
+    const long long v = vrow(k);
+    float* dst = v < nU ? g.pf_nc + v * (long long)g.D : g.pf_bn + (v - nU) * (long long)g.D;
+    const long long kr = k - L + S;                // the item that takes over the slot of item k - L
+    const bool reload = k >= L && kr < n;
+    // rotate the id window one batch early: the fresh batch is needed 32 items from now
+    if (reload && kr >= base + 32) { base += 32; ids_lo = ids_hi; ids_hi = fetch_ids(base + 32); }
+    if (elect_one()) {
+      bulk_s2g(dst, slots + (size_t)s * g.pf_row_bytes, g.pf_row_bytes);
+      bulk_commit();
+      if (reload) { if (L == 3) bulk_wait_read<3>(); else if (L == 2) bulk_wait_read<2>(); else bulk_wait_read<1>(); }
+    }
+    __syncwarp();
+    if (reload) load(kr);
+  }
+  if (elect_one()) bulk_wait_all();
+  __syncwarp();
+}
+
+// ================================ k_fused<P> ================================
+template <int NV>
 __global__ void __launch_bounds__(kThreadsF, 1)
-k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtensorMap mXl,
-        const __grid_constant__ CUtensorMap mYh1, const __grid_constant__ CUtensorMap mYl1,
-        const __grid_constant__ CUtensorMap mYh2, const __grid_constant__ CUtensorMap mYl2, FusedArgs g) {
+k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtensorMap mXl,
+            const __grid_constant__ CUtensorMap mYh1, const __grid_constant__ CUtensorMap mYl1,
+            const __grid_constant__ CUtensorMap mYh2, const __grid_constant__ CUtensorMap mYl2, FusedArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full1[kMaxS1], empty1[kMaxS1], full2[kMaxS2], empty2[kMaxS2];
   __shared__ __align__(8) uint64_t pf_full[2][kMaxPf];
-  __shared__ __align__(16) float colA[NV], colB[NV], colC[NV];
+  __shared__ __align__(16) float colA[NV];
+  __shared__ __align__(16) float cpart[8][NV];     // column sums of V over the 16 rows of each MMA warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint8_t* ring = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -183,61 +242,7 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
       }
     }
   } else if (warp >= 10 && g.pf_slots > 0) {
-    // ================================ prefetch warps 10, 11 ================================
-    // Each warp streams table rows (peer memory when the table is sharded) through a few shared-memory slots into the
-    // next step's buffers: bulk load -> mbarrier -> bulk store, S slots per warp re-used round robin.  The loop is warp-uniform (one
-    // elected lane issues): the row ids arrive 32 at a time, one coalesced load per lane, and are handed out by shuffle
-    // -- a per-row dependent id load by a single lane costs more than the copy itself.
-    const int w = warp - 10, S = g.pf_slots;
-    const long long nU = g.pf_nU_dev ? *g.pf_nU_dev : g.pf_nU;
-    const long long total = nU + g.pf_nNeg;
-    const long long nhalf = total > g.pf_parity ? (total - g.pf_parity + 1) / 2 : 0;   // v = parity + 2 j < total
-    const long long stride = 2ll * gridDim.x, j0 = 2ll * blockIdx.x + w;
-    const long long n = j0 < nhalf ? (nhalf - j0 + stride - 1) / stride : 0;
-    uint8_t* slots = ring + g.pf_off + (size_t)w * S * g.pf_row_bytes;
-    auto vrow = [&](long long k) { return g.pf_parity + 2 * (j0 + k * stride); };
-    auto fetch_ids = [&](long long kb) {            // ids of items kb .. kb+31, one per lane
-      const long long k = kb + lane;
-      if (k >= n) return 0ll;
-      const long long v = vrow(k);
-      return v < nU ? g.pf_node_ids[v] : g.pf_neg_ids[v - nU];
-    };
-    long long ids_lo = fetch_ids(0), ids_hi = fetch_ids(32);      // items [base, base+32) and [base+32, base+64)
-    long long base = 0;
-    auto load = [&](long long k) {                  // k in [base, base + 64)
-      const int o = (int)(k - base);
-      const long long id = __shfl_sync(0xffffffffu, o < 32 ? ids_lo : ids_hi, o & 31);
-      const int s = (int)(k % S);
-      if (elect_one()) {
-        mbar_expect_tx(&pf_full[w][s], g.pf_row_bytes);
-        bulk_g2s(slots + (size_t)s * g.pf_row_bytes, row_ptr(g.xtab, id), g.pf_row_bytes, &pf_full[w][s]);
-      }
-      __syncwarp();
-    };
-    for (long long k = 0; k < n && k < S; ++k) load(k);
-    // A slot is re-loaded L stores after its own store was issued (S - L loads in flight).  L = 1 keeps the most loads in
-    // flight, which is what matters when the rows are remote; a larger L (KGE_B200_PF_LAG) never waits on the copy
-    // engine's queue for the newest store.
-    const int L = g.pf_lag < S - 1 ? g.pf_lag : (S > 2 ? S - 2 : 1);
-    for (long long k = 0; k < n; ++k) {
-      const int s = (int)(k % S);
-      mbar_wait(&pf_full[w][s], (uint32_t)((k / S) & 1));
-      const long long v = vrow(k);
-      float* dst = v < nU ? g.pf_nc + v * (long long)g.D : g.pf_bn + (v - nU) * (long long)g.D;
-      const long long kr = k - L + S;                // the item that takes over the slot of item k - L
-      const bool reload = k >= L && kr < n;
-      // rotate the id window one batch early: the fresh batch is needed 32 items from now
-      if (reload && kr >= base + 32) { base += 32; ids_lo = ids_hi; ids_hi = fetch_ids(base + 32); }
-      if (elect_one()) {
-        bulk_s2g(dst, slots + (size_t)s * g.pf_row_bytes, g.pf_row_bytes);
-        bulk_commit();
-        if (reload) { if (L == 3) bulk_wait_read<3>(); else if (L == 2) bulk_wait_read<2>(); else bulk_wait_read<1>(); }
-      }
-      __syncwarp();
-      if (reload) load(kr);
-    }
-    if (elect_one()) bulk_wait_all();
-    __syncwarp();
+    prefetch_rows(g, ring, pf_full, warp - 10, lane);
   }
   } else {
     // ================================ MMA + epilogue warps 0..7 ================================
@@ -252,9 +257,7 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
       epi_bar();                                  // everybody is done with the previous tile's shared constants
       for (int y = et; y < NV; y += 256) {
         const bool ok = y < g.Ry;
-        const long long gy = (long long)c * g.Ry + y;
-        colA[y] = (l2 && ok) ? g.y2[gy] : 0.f;
-        if (MODE == F_N) { colB[y] = ok ? g.cstat_m[gy] : 0.f; colC[y] = ok ? g.cstat_k[gy] : 0.f; }
+        colA[y] = (l2 && ok) ? g.y2[(long long)c * g.Ry + y] : 0.f;
       }
       epi_bar();
       // ---- GEMM1: S = X . Y^T, K = D ----
@@ -286,130 +289,131 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
       reg_fence(acc);
 
       // ---- S -> V in place, two rows per thread; a row's statistics are reduced over the 4 lanes of its quad ----
-      float rscal[2];                             // mode P: 1 / softmax denominator; mode N: colsum (TransE_l2)
+      float rscal[2];                             // 1 / softmax denominator (or 1 / Ns) of the two rows
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int m = m0 + rloc + 8 * h;
         const bool row_ok = m < g.Rx;
         const long long gx = (long long)c * g.Rx + (row_ok ? m : 0);
         const float x2v = (l2 && row_ok) ? g.x2[gx] : 0.f;
-        if (MODE == F_P) {
-          const float w_i = (g.wt && row_ok) ? g.wt[gx] : 1.f;
-          const float kw = w_i * g.inv2B;
-          // ---- pass A: scores (distance epilogue for TransE_l2), running max ----
-          float mxl = -INFINITY;
-          if (g.adversarial || g.dumpS) {
-#pragma unroll
-            for (int j = 0; j < NV / 8; ++j) {
-              float sv[2];
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int col = 8 * j + 2 * q + e;
-                float s = acc[4 * j + 2 * h + e];
-                if (l2) {
-                  // batched_l2_dist (score_fun.py:26-34): (|b|^2 - 2 a.b) + |a|^2, clamp 1e-30, sqrt
-                  const float sqc = fmaxf(fmaf(-2.f, s, colA[col]) + x2v, 1e-30f);
-                  s = g.gamma - sqc * rsqrta(sqc);
-                }
-                sv[e] = s;
-                if (col < g.Ry) mxl = fmaxf(mxl, s * g.Tl2e);
-              }
-              if (g.dumpS && row_ok && 8 * j + 2 * q < g.Ry)
-                *reinterpret_cast<float2*>(g.dumpS + gx * g.Ry + 8 * j + 2 * q) = make_float2(sv[0], sv[1]);
-            }
-          }
-          if (g.adversarial) {
-            mxl = fmaxf(mxl, __shfl_xor_sync(0xffffffffu, mxl, 1));
-            mxl = fmaxf(mxl, __shfl_xor_sync(0xffffffffu, mxl, 2));
-          } else {
-            mxl = 0.f;
-          }
-          // ---- pass C: softmax numerators, loss terms and (unnormalised) backward coefficients.  The 1/denominator of
-          //      the row is a per-row scalar: it is applied to the loss sums here and to the row of GA in the GEMM2
-          //      epilogue. ----
-          float nls = 0.f, rs = 0.f, den = 0.f;
+        const float w_i = (g.wt && row_ok) ? g.wt[gx] : 1.f;
+        const float kw = w_i * g.inv2B;
+        // ---- pass A: scores (distance epilogue for TransE_l2), running max ----
+        float mxl = -INFINITY;
+        if (g.adversarial || g.dumpS) {
 #pragma unroll
           for (int j = 0; j < NV / 8; ++j) {
+            float sv[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int col = 8 * j + 2 * q + e;
-              float s = acc[4 * j + 2 * h + e], rinv = 1.f;
+              float s = acc[4 * j + 2 * h + e];
               if (l2) {
-                const float sq = fmaf(-2.f, s, colA[col]) + x2v;
-                const float sqc = fmaxf(sq, 1e-30f);
-                const float r = rsqrta(sqc);
-                s = g.gamma - sqc * r;
-                rinv = (sq > 1e-30f) ? r : 0.f;        // clamped distance: zero gradient (clamp_min_), dist ~ 0
+                // batched_l2_dist (score_fun.py:26-34): (|b|^2 - 2 a.b) + |a|^2, clamp 1e-30, sqrt
+                const float sqc = fmaxf(fmaf(-2.f, s, colA[col]) + x2v, 1e-30f);
+                s = g.gamma - sqc * rsqrta(sqc);
               }
-              const float pe = g.adversarial ? ex2a(fmaf(s, g.Tl2e, -mxl)) : 1.f;
-              const float t = ex2a(-fabsf(s) * kLog2e);
-              const float u = 1.f + t;
-              const float r1 = rcpa(u);
-              const float sig = (s >= 0.f) ? r1 : t * r1;                     // sigmoid(s)
-              const float sp = fmaf(kLn2, lg2a(u), fmaxf(s, 0.f));            // -logsigmoid(-s)
-              const bool ok = row_ok && (col < g.Ry);
-              const float coef = ok ? pe * sig * kw * rinv : 0.f;              // dL/dneg_ij (/ dist) * denominator
-              if (ok) { nls = fmaf(pe, sp, nls); den += pe; }
-              rs += coef;
-              acc[4 * j + 2 * h + e] = coef;
+              sv[e] = s;
+              if (col < g.Ry) mxl = fmaxf(mxl, s * g.Tl2e);
             }
+            if (g.dumpS && row_ok && 8 * j + 2 * q < g.Ry)
+              *reinterpret_cast<float2*>(g.dumpS + gx * g.Ry + 8 * j + 2 * q) = make_float2(sv[0], sv[1]);
           }
-          den += __shfl_xor_sync(0xffffffffu, den, 1); den += __shfl_xor_sync(0xffffffffu, den, 2);
-          nls += __shfl_xor_sync(0xffffffffu, nls, 1); nls += __shfl_xor_sync(0xffffffffu, nls, 2);
-          rs += __shfl_xor_sync(0xffffffffu, rs, 1); rs += __shfl_xor_sync(0xffffffffu, rs, 2);
-          const float rscale = g.adversarial ? (row_ok ? 1.f / den : 0.f) : g.uni;
-          rscal[h] = rscale;
-          if (g.dumpV && row_ok) {        // test hook: the dump shows the normalised coefficients
-#pragma unroll
-            for (int j = 0; j < NV / 8; ++j)
-              if (8 * j + 2 * q < g.Ry)
-                *reinterpret_cast<float2*>(g.dumpV + gx * g.Ry + 8 * j + 2 * q) =
-                    make_float2(acc[4 * j + 2 * h] * rscale, acc[4 * j + 2 * h + 1] * rscale);
-          }
-          if (q == 0 && row_ok) {
-            const float ps = g.pos[gx];
-            const float wb = g.wt ? *g.wbar : 1.f;        // loss.py:75,82: [B] * [B,1] -> mean(pl) * mean(w)
-            g.pl[gx] = softplusf(-ps);
-            g.nl[gx] = nls * rscale * w_i;
-            g.gpos[gx] = -sigmoidf(-ps) * wb * g.inv2B;
-            if (l2) g.rowsum[gx] = rs * rscale;
-            g.stat_m[gx] = mxl;
-            g.stat_k[gx] = kw * rscale;
-          }
+        }
+        if (g.adversarial) {
+          mxl = fmaxf(mxl, __shfl_xor_sync(0xffffffffu, mxl, 1));
+          mxl = fmaxf(mxl, __shfl_xor_sync(0xffffffffu, mxl, 2));
         } else {
-          // ---- mode N: one pass, the softmax statistics of every column (positive) come from mode P ----
-          float cs = 0.f;
+          mxl = 0.f;
+        }
+        // ---- pass C: softmax numerators, loss terms and (unnormalised) backward coefficients.  The 1/denominator of
+        //      the row is a per-row scalar: it is applied to the loss sums here and to the row of GA in the GEMM2
+        //      epilogue. ----
+        float nls = 0.f, rs = 0.f, den = 0.f;
+#pragma unroll
+        for (int j = 0; j < NV / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * j + 2 * q + e;
+            float s = acc[4 * j + 2 * h + e], rinv = 1.f;
+            if (l2) {
+              const float sq = fmaf(-2.f, s, colA[col]) + x2v;
+              const float sqc = fmaxf(sq, 1e-30f);
+              const float r = rsqrta(sqc);
+              s = g.gamma - sqc * r;
+              rinv = (sq > 1e-30f) ? r : 0.f;        // clamped distance: zero gradient (clamp_min_), dist ~ 0
+            }
+            const float pe = g.adversarial ? ex2a(fmaf(s, g.Tl2e, -mxl)) : 1.f;
+            const float t = ex2a(-fabsf(s) * kLog2e);
+            const float u = 1.f + t;
+            const float r1 = rcpa(u);
+            const float sig = (s >= 0.f) ? r1 : t * r1;                     // sigmoid(s)
+            const float sp = fmaf(kLn2, lg2a(u), fmaxf(s, 0.f));            // -logsigmoid(-s)
+            const bool ok = row_ok && (col < g.Ry);
+            const float coef = ok ? pe * sig * kw * rinv : 0.f;              // dL/dneg_ij (/ dist) * denominator
+            if (ok) { nls = fmaf(pe, sp, nls); den += pe; }
+            rs += coef;
+            acc[4 * j + 2 * h + e] = coef;
+          }
+        }
+        den += __shfl_xor_sync(0xffffffffu, den, 1); den += __shfl_xor_sync(0xffffffffu, den, 2);
+        nls += __shfl_xor_sync(0xffffffffu, nls, 1); nls += __shfl_xor_sync(0xffffffffu, nls, 2);
+        rs += __shfl_xor_sync(0xffffffffu, rs, 1); rs += __shfl_xor_sync(0xffffffffu, rs, 2);
+        const float rscale = g.adversarial ? (row_ok ? 1.f / den : 0.f) : g.uni;
+        rscal[h] = rscale;
+        if (g.dumpV && row_ok) {        // test hook: the dump shows the normalised coefficients
+#pragma unroll
+          for (int j = 0; j < NV / 8; ++j)
+            if (8 * j + 2 * q < g.Ry)
+              *reinterpret_cast<float2*>(g.dumpV + gx * g.Ry + 8 * j + 2 * q) =
+                  make_float2(acc[4 * j + 2 * h] * rscale, acc[4 * j + 2 * h + 1] * rscale);
+        }
+        // ---- hand V to k_fused<N>: V_ij = coef_ij / den_i as TF32 hi/lo in the transposed slabs
+        //      V^T[c][i / 32][j][i % 32].  The 8 lanes that share q hold 8 consecutive i of the same j, so every store
+        //      fills a whole 32-byte sector; rows i >= Cs and columns j >= Ns are not written (k_fused<N> never reads
+        //      them).  TransE_l2 also needs sum_i V_ij: summed over the 16 rows of the warp by shuffles and the two
+        //      rows of the thread in cpart, then over the 8 warps after the loop. ----
+        {
+          float* vh = g.VhiT + slabT_off(c, g.Rx, g.Ry, m, 0);
+          float* vl = g.VloT + slabT_off(c, g.Rx, g.Ry, m, 0);
 #pragma unroll
           for (int j = 0; j < NV / 8; ++j) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int col = 8 * j + 2 * q + e;
-              float s = acc[4 * j + 2 * h + e], rinv = 1.f;
-              if (l2) {
-                const float sq = fmaf(-2.f, s, x2v) + colA[col];
-                const float sqc = fmaxf(sq, 1e-30f);
-                const float r = rsqrta(sqc);
-                s = g.gamma - sqc * r;
-                rinv = (sq > 1e-30f) ? r : 0.f;
+              const float v = acc[4 * j + 2 * h + e] * rscale;
+              if (row_ok && col < g.Ry) {
+                float hi, lo;
+                split_tf32(v, hi, lo);
+                vh[col * 32] = hi; vl[col * 32] = lo;
               }
-              const float pe = g.adversarial ? ex2a(fmaf(s, g.Tl2e, -colB[col])) : 1.f;
-              const float t = ex2a(-fabsf(s) * kLog2e);
-              const float r1 = rcpa(1.f + t);
-              const float sig = (s >= 0.f) ? r1 : t * r1;
-              float coef = pe * colC[col] * sig * rinv;
-              if (!(row_ok && (col < g.Ry))) coef = 0.f;
-              cs += coef;
-              acc[4 * j + 2 * h + e] = coef;
+              if (l2) {
+                float s = v;
+                s += __shfl_xor_sync(0xffffffffu, s, 4);
+                s += __shfl_xor_sync(0xffffffffu, s, 8);
+                s += __shfl_xor_sync(0xffffffffu, s, 16);
+                if (lane < 4) cpart[warp][col] = h ? cpart[warp][col] + s : s;
+              }
             }
           }
-          cs += __shfl_xor_sync(0xffffffffu, cs, 1); cs += __shfl_xor_sync(0xffffffffu, cs, 2);
-          rscal[h] = cs;
-          if (g.dumpV && row_ok) {
+        }
+        if (q == 0 && row_ok) {
+          const float ps = g.pos[gx];
+          const float wb = g.wt ? *g.wbar : 1.f;        // loss.py:75,82: [B] * [B,1] -> mean(pl) * mean(w)
+          g.pl[gx] = softplusf(-ps);
+          g.nl[gx] = nls * rscale * w_i;
+          g.gpos[gx] = -sigmoidf(-ps) * wb * g.inv2B;
+          if (l2) g.rowsum[gx] = rs * rscale;
+        }
+      }
+      if (l2) {
+        epi_bar();                                // every warp's column sums are in cpart
+        float* dst = g.colpart + (long long)(tile % mtiles) * g.C * g.Ry + (long long)c * g.Ry;
+        for (int y = et; y < g.Ry; y += 256) {
+          float s = cpart[0][y];
 #pragma unroll
-            for (int j = 0; j < NV / 8; ++j)
-              if (8 * j + 2 * q < g.Ry)
-                *reinterpret_cast<float2*>(g.dumpV + gx * g.Ry + 8 * j + 2 * q) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-          }
+          for (int w = 1; w < 8; ++w) s += cpart[w][y];
+          dst[y] = s;
         }
       }
       // ---- accumulator fragment -> register A fragment of GEMM2: within every group of 8 columns a thread holds columns
@@ -433,8 +437,7 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
         }
       }
 
-      // ---- GEMM2: G[:, chunk] = V . Y[:, chunk], K = Ry, A operand from registers; epilogue per 128-column chunk ----
-      float gsq[2] = {0.f, 0.f};
+      // ---- GEMM2: GA[:, chunk] = V . Bn[:, chunk], K = Ns, A operand from registers; epilogue per 128-column chunk ----
       for (int ch = 0; ch < nchunks; ++ch) {
         const int d0 = ch * kWc;
         float acc2[kWc / 2];
@@ -483,48 +486,195 @@ k_fused(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtenso
         for (int h = 0; h < 2; ++h) {
           const int m = m0 + rloc + 8 * h;
           if (m >= g.Rx) continue;
-          const long long gx = (long long)c * g.Rx + m;
-          float* orow = g.out + gx * (long long)g.D;
-          const float* brow = nullptr;
-          if (MODE == F_N) brow = g.xraw ? g.xraw + gx * (long long)g.D : (g.xids ? row_ptr(g.xtab, g.xids[gx]) : nullptr);
+          float* orow = g.out + ((long long)c * g.Rx + m) * (long long)g.D;
 #pragma unroll
           for (int j = 0; j < kWc / 8; ++j) {
             const int k = d0 + 8 * j + 2 * q;
             if (k >= g.D) continue;
-            float o0 = acc2[4 * j + 2 * h], o1 = acc2[4 * j + 2 * h + 1];
-            if (MODE == F_P) { o0 *= rscal[h]; o1 *= rscal[h]; }          // 1 / softmax denominator of the row
-            if (MODE == F_N) {
-              float2 b;
-              if (brow) b = *reinterpret_cast<const float2*>(brow + k);
-              else {
-                const long long so = slab_off(c, g.nblkD, g.Rx, m, k);
-                const float2 bh = *reinterpret_cast<const float2*>(g.Xhi + so), bl = *reinterpret_cast<const float2*>(g.Xlo + so);
-                b = make_float2(bh.x + bl.x, bh.y + bl.y);
-              }
-              if (l2) { o0 = fmaf(b.x, -rscal[h], o0); o1 = fmaf(b.y, -rscal[h], o1); }   // sum_i V_ij a_i - (sum_i V_ij) b_j
-              o0 += reg_grad_fast(b.x, g.reg_norm, g.reg_coef);
-              o1 += reg_grad_fast(b.y, g.reg_norm, g.reg_coef);
-              gsq[h] += o0 * o0 + o1 * o1;
-            }
-            *reinterpret_cast<float2*>(orow + k) = make_float2(o0, o1);
+            // 1 / softmax denominator of the row
+            *reinterpret_cast<float2*>(orow + k) = make_float2(acc2[4 * j + 2 * h] * rscal[h], acc2[4 * j + 2 * h + 1] * rscal[h]);
           }
-        }
-      }
-      if (MODE == F_N) {
-        // mean(G_neg^2) per row: the 4 lanes that share a row
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float v = gsq[h];
-          v += __shfl_xor_sync(0xffffffffu, v, 1);
-          v += __shfl_xor_sync(0xffffffffu, v, 2);
-          const int m = m0 + rloc + 8 * h;
-          if (q == 0 && m < g.Rx) g.gsn[(long long)c * g.Rx + m] = v / (float)g.D;
         }
       }
     }
   }
 }
 
+// ================================ k_fused<N> ================================
+// one k-block of G_neg: KS k-steps of 8, each hi*hi + hi*lo + lo*hi, as one wgmma group
+template <int NW, int KS>
+__device__ __forceinline__ void neg_kblock(float (&acc)[NW / 2], uint64_t dVh, uint64_t dVl, uint64_t dAh, uint64_t dAl) {
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    const uint64_t o = (uint64_t)(ks * 2);     // K-major: +32 bytes per k-step inside the 128-byte swizzle span
+    wgmma_ss<NW>(acc, dVh + o, dAh + o, 1u);
+    wgmma_ss<NW>(acc, dVh + o, dAl + o, 1u);
+    wgmma_ss<NW>(acc, dVl + o, dAh + o, 1u);
+  }
+  wgmma_commit();
+}
+
+// G_neg[c][j, d0 : d0 + NW] = sum_i V^T[j, i] A[i, d0 : d0 + NW] for one 128-row tile of negatives j and one output
+// chunk of NW columns per pass over K = Cs; the stages carry the tile's V^T k-block and the chunk's A^T k-block.
+template <int NW>
+__global__ void __launch_bounds__(kThreadsF, 1)
+k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUtensorMap mVl,
+            const __grid_constant__ CUtensorMap mAh, const __grid_constant__ CUtensorMap mAl, FusedArgs g) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full[kMaxS1], empty[kMaxS1];
+  __shared__ __align__(8) uint64_t pf_full[2][kMaxPf];
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint8_t* ring = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+
+  const int mtiles = (g.Rx + kTileM - 1) / kTileM;
+  const int ntiles = g.C * mtiles;
+  const int nkb = (g.Ry + 31) >> 5;               // k-blocks of K = Cs
+  const int nch = (g.D + NW - 1) / NW;
+  constexpr uint32_t aBytes = (uint32_t)kTileM * 128u;
+  constexpr uint32_t bBytes = (uint32_t)NW * 128u;
+  const bool l2 = g.model == KGE_TRANSE_L2;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kMaxS1; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    for (int s = 0; s < kMaxPf; ++s) { mbar_init(&pf_full[0][s], 1); mbar_init(&pf_full[1][s], 1); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (warp == kProducerWarp && lane == 0) {
+    tma_prefetch_desc(&mVh); tma_prefetch_desc(&mVl); tma_prefetch_desc(&mAh); tma_prefetch_desc(&mAl);
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+  if (warp == kProducerWarp) {
+    // ================================ TMA producer ================================
+    uint32_t n = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      const int c = tile / mtiles, m0 = (tile % mtiles) * kTileM;
+      for (int ch = 0; ch < nch; ++ch) {
+        for (int kb = 0; kb < nkb; ++kb, ++n) {
+          const uint32_t s = n % g.nS1;
+          mbar_wait(&empty[s], ((n / g.nS1) & 1) ^ 1);
+          uint8_t* st = ring + (size_t)s * g.stage1Bytes;
+          // transposed slabs: TMA row of (chunk c, 32-row block kb, column) = (c * nkb + kb) * columns + column
+          const int yv = (c * nkb + kb) * g.Rx + m0;
+          const int ya = (c * nkb + kb) * g.D + ch * NW;
+          if (elect_one()) {
+            mbar_expect_tx(&full[s], 2u * aBytes + 2u * bBytes);
+            tma_load_2d(st, &mVh, &full[s], 0, yv);
+            tma_load_2d(st + aBytes, &mVl, &full[s], 0, yv);
+            tma_load_2d(st + 2 * aBytes, &mAh, &full[s], 0, ya);
+            tma_load_2d(st + 2 * aBytes + bBytes, &mAl, &full[s], 0, ya);
+          }
+          __syncwarp();
+        }
+      }
+    }
+  } else if (warp >= 10 && g.pf_slots > 0) {
+    prefetch_rows(g, ring, pf_full, warp - 10, lane);
+  }
+  } else {
+    // ================================ MMA + epilogue warps 0..7 ================================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+    const int wg = warp >> 2, q = lane & 3;
+    const int et = threadIdx.x;                   // 0..255
+    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread's rows inside the tile: rloc, rloc + 8
+    uint32_t n = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      const int c = tile / mtiles, m0 = (tile % mtiles) * kTileM;
+      if (g.dumpV) {
+        // test hook: the coefficients this tile reads, [C*Ns, Cs] (hi + lo)
+        for (int e = et; e < kTileM * g.Ry; e += 256) {
+          const int j = m0 + e / g.Ry, i = e % g.Ry;
+          if (j >= g.Rx) break;
+          const long long o = slabT_off(c, g.Ry, g.Rx, i, j);
+          g.dumpV[((long long)c * g.Rx + j) * g.Ry + i] = g.VhiT[o] + g.VloT[o];
+        }
+      }
+      // sum_i V_ij of this thread's two rows: the per-tile partials of k_fused<P>, added in a fixed order
+      float cs[2] = {0.f, 0.f};
+      if (l2) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = m0 + rloc + 8 * h;
+          if (m >= g.Rx) continue;
+          const float* p = g.colpart + (long long)c * g.Rx + m;
+          for (int t = 0; t < g.ncolpart; ++t) cs[h] += p[(long long)t * g.C * g.Rx];
+        }
+      }
+      float gsq[2] = {0.f, 0.f};
+      for (int ch = 0; ch < nch; ++ch) {
+        const int d0 = ch * NW;
+        float acc[NW / 2];                        // rows rloc (+8), columns d0 + 8 j + 2 q + {0, 1}
+#pragma unroll
+        for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < nkb; ++kb, ++n) {
+          const uint32_t s = n % g.nS1;
+          mbar_wait(&full[s], (n / g.nS1) & 1);
+          const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
+          const uint64_t dVh = make_desc(st + wg * 8192u), dVl = make_desc(st + aBytes + wg * 8192u);
+          const uint64_t dAh = make_desc(st + 2 * aBytes), dAl = make_desc(st + 2 * aBytes + bBytes);
+          // K = Cs is a multiple of 8: the partial last block runs its whole k-steps and never reads the padding
+          const int kleft = g.Ry - kb * 32;
+          const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
+          // one straight-line fence .. wgmma .. commit sequence per k-step count: a guard between the fence and the
+          // commit makes ptxas insert warpgroup arrives of its own
+          switch (ksteps) {
+            case 4: neg_kblock<NW, 4>(acc, dVh, dVl, dAh, dAl); break;
+            case 3: neg_kblock<NW, 3>(acc, dVh, dVl, dAh, dAl); break;
+            case 2: neg_kblock<NW, 2>(acc, dVh, dVl, dAh, dAl); break;
+            default: neg_kblock<NW, 1>(acc, dVh, dVl, dAh, dAl); break;
+          }
+          if (kb > 0) {
+            wgmma_wait<1>();                           // the previous k-block has retired: its stage is free
+            if (lane == 0) mbar_arrive(&empty[(n - 1) % g.nS1]);
+          }
+        }
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&empty[(n - 1) % g.nS1]);
+        reg_fence(acc);
+        // chunk epilogue from the fragment (the producer is already filling the next chunk's stages)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = m0 + rloc + 8 * h;
+          if (m >= g.Rx) continue;
+          const long long gx = (long long)c * g.Rx + m;
+          float* orow = g.out + gx * (long long)g.D;
+          const float* brow = g.xraw ? g.xraw + gx * (long long)g.D : (g.xids ? row_ptr(g.xtab, g.xids[gx]) : nullptr);
+#pragma unroll
+          for (int j = 0; j < NW / 8; ++j) {
+            const int k = d0 + 8 * j + 2 * q;
+            if (k >= g.D) continue;
+            float o0 = acc[4 * j + 2 * h], o1 = acc[4 * j + 2 * h + 1];
+            float2 b;
+            if (brow) b = *reinterpret_cast<const float2*>(brow + k);
+            else {
+              const long long so = slab_off(c, g.nblkD, g.Rx, m, k);
+              const float2 bh = *reinterpret_cast<const float2*>(g.Xhi + so), bl = *reinterpret_cast<const float2*>(g.Xlo + so);
+              b = make_float2(bh.x + bl.x, bh.y + bl.y);
+            }
+            if (l2) { o0 = fmaf(b.x, -cs[h], o0); o1 = fmaf(b.y, -cs[h], o1); }   // sum_i V_ij a_i - (sum_i V_ij) b_j
+            o0 += reg_grad_fast(b.x, g.reg_norm, g.reg_coef);
+            o1 += reg_grad_fast(b.y, g.reg_norm, g.reg_coef);
+            gsq[h] += o0 * o0 + o1 * o1;
+            *reinterpret_cast<float2*>(orow + k) = make_float2(o0, o1);
+          }
+        }
+      }
+      // mean(G_neg^2) per row: the 4 lanes that share a row
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v = gsq[h];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        const int m = m0 + rloc + 8 * h;
+        if (q == 0 && m < g.Rx) g.gsn[(long long)c * g.Rx + m] = v / (float)g.D;
+      }
+    }
+  }
+}
 
 }  // namespace
 
@@ -535,14 +685,48 @@ bool fused_supported(const StepParams& p) {
   return umma_supported(p) && !p.hinge && !p.pairwise && !p.neg_deg && p.Cs <= 240 && p.Ns <= 240;
 }
 
-// mode 0 (P): S = A.Bn^T -> loss, coefficients -> GA;  mode 1 (N): S^T -> coefficients -> G_neg (+ mean square)
+// mode 0 (P): S = A.Bn^T -> loss, coefficients V -> GA, V^T slabs;  mode 1 (N): G_neg = V^T.A (+ mean square)
 namespace {
 // GEMM stage geometry of one mode + what the ring leaves for prefetch row slots
 struct Geometry { int Rx, Ry, N1, nS1, nS2, pf_slots; uint32_t stage1Bytes, stage2Bytes, pf_off; bool ok; };
+
+// k_fused<N>: the output-column chunk NW.  A pass over K streams the tile's V^T (128 rows) and the chunk's A^T (NW rows),
+// 128 B per row and k-block, so a CTA streams nch * (128 + NW) rows per k-block for nch = ceil(D / NW) chunks: the
+// width with the fewest is taken (d = 400: 2 x 200 -> 656 rows, against 768 for 2 x 256 and 1024 for 4 x 128).  A
+// 256-wide stage (96 KB) fills the ring twice over, so it is not offered when prefetch slots are wanted.
+int neg_chunk_width(int D, bool want_prefetch) {
+  static const int widths[] = {64, 128, 200, 256};
+  int best = 0;
+  long long best_rows = 0;
+  for (int w : widths) {
+    if (w == 256 && want_prefetch) continue;
+    const long long rows = (long long)((D + w - 1) / w) * (kTileM + w);
+    if (!best || rows < best_rows) { best = w; best_rows = rows; }
+  }
+  return best;
+}
+
 Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
   Geometry q{};
-  const bool P = mode == 0;
-  q.Rx = P ? p.Cs : p.Ns; q.Ry = P ? p.Ns : p.Cs;
+  const uint32_t row = (uint32_t)p.D * 4u;
+  if (mode == 1) {
+    q.Rx = p.Ns; q.Ry = p.Cs;
+    q.N1 = neg_chunk_width(p.D, want_prefetch);
+    q.stage1Bytes = 2u * kTileM * 128u + 2u * (uint32_t)q.N1 * 128u;
+    q.nS1 = (int)(kRingBytes / q.stage1Bytes); if (q.nS1 > kMaxS1) q.nS1 = kMaxS1;
+    q.ok = q.nS1 >= 2;
+    if (q.ok && want_prefetch) {
+      // the GEMM gives up stages (never below 2) until both prefetch warps have kMaxPf row slots
+      int nS = q.nS1;
+      while (nS > 2 && kRingBytes - (uint32_t)nS * q.stage1Bytes < 2u * kMaxPf * row) --nS;
+      const uint32_t used = (uint32_t)nS * q.stage1Bytes;
+      int slots = (int)((kRingBytes - used) / (2u * row));
+      if (slots > kMaxPf) slots = kMaxPf;
+      if (slots >= 2) { q.pf_slots = slots; q.nS1 = nS; q.pf_off = used; }
+    }
+    return q;
+  }
+  q.Rx = p.Cs; q.Ry = p.Ns;
   // wgmma's N is part of the instruction: the kernel is instantiated for these widths
   q.N1 = q.Ry <= 64 ? 64 : (q.Ry <= 128 ? 128 : (q.Ry <= 208 ? 208 : 256));
   q.stage1Bytes = 2u * 16384u + 2u * (uint32_t)q.N1 * 128u;
@@ -552,7 +736,6 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
   q.ok = q.nS1 >= 2 && q.nS2 >= 2;
   if (q.ok && want_prefetch) {
     // GEMM1 keeps its stages; GEMM2 gives up stages (never below 4) until both prefetch warps have kMaxPf row slots
-    const uint32_t row = (uint32_t)p.D * 4u;
     int nS1 = q.nS1, nS2 = q.nS2;
     uint32_t want = 2u * kMaxPf * row;
     while (nS1 > 2 && kRingBytes - (uint32_t)nS1 * q.stage1Bytes < want) --nS1;   // a deep GEMM1 ring gives up stages first
@@ -567,21 +750,30 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
   return q;
 }
 
-template <int MODE, int NV>
-int launch_variant(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
-  if (int rc = smem_optin((const void*)k_fused<MODE, NV>, smem)) return rc;
-  KGE_LAUNCH_NAMED(c, MODE == F_P ? "k_fused<P: S=A.Bn^T, loss, GA=V.Bn>" : "k_fused<N: S^T, G_neg=V^T.A, mean sq>",
-                   (k_fused<MODE, NV>), grid, kThreadsF, smem, m[0], m[1], m[2], m[3], m[4], m[5], g);
+int launch_error() {
   const cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? KGE_OK : fail(KGE_ERR_CUDA, "k_fused launch: %s", cudaGetErrorString(e));
 }
-template <int MODE>
-int launch_width(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+template <int NV>
+int launch_pos(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+  if (int rc = smem_optin((const void*)k_fused_pos<NV>, smem)) return rc;
+  KGE_LAUNCH_NAMED(c, "k_fused<P: S=A.Bn^T, loss, GA=V.Bn>", (k_fused_pos<NV>), grid, kThreadsF, smem,
+                   m[0], m[1], m[2], m[3], m[4], m[5], g);
+  return launch_error();
+}
+template <int NW>
+int launch_neg(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+  if (int rc = smem_optin((const void*)k_fused_neg<NW>, smem)) return rc;
+  KGE_LAUNCH_NAMED(c, "k_fused<N: G_neg=V^T.A, mean sq>", (k_fused_neg<NW>), grid, kThreadsF, smem, m[0], m[1], m[2], m[3], g);
+  return launch_error();
+}
+int launch_width(const LaunchCtx& c, bool P, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
   switch (g.N1) {
-    case 64: return launch_variant<MODE, 64>(c, grid, smem, m, g);
-    case 128: return launch_variant<MODE, 128>(c, grid, smem, m, g);
-    case 208: return launch_variant<MODE, 208>(c, grid, smem, m, g);
-    default: return launch_variant<MODE, 256>(c, grid, smem, m, g);
+    case 64: return P ? launch_pos<64>(c, grid, smem, m, g) : launch_neg<64>(c, grid, smem, m, g);
+    case 128: return P ? launch_pos<128>(c, grid, smem, m, g) : launch_neg<128>(c, grid, smem, m, g);
+    case 200: return launch_neg<200>(c, grid, smem, m, g);
+    case 208: return launch_pos<208>(c, grid, smem, m, g);
+    default: return P ? launch_pos<256>(c, grid, smem, m, g) : launch_neg<256>(c, grid, smem, m, g);
   }
 }
 }  // namespace
@@ -608,33 +800,41 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
     g.pf_neg_ids = pf->neg_ids; g.pf_nc = pf->nc; g.pf_bn = pf->bn;
     g.xtab = *ent;
   }
-  const float *Xh = P ? w.Ahi : w.Bhi, *Xl = P ? w.Alo : w.Blo, *Yh = P ? w.Bhi : w.Ahi, *Yl = P ? w.Blo : w.Alo;
-  g.x2 = P ? w.a2 : w.b2; g.y2 = P ? w.b2 : w.a2;
-  g.pos = w.pos; g.wt = wt; g.wbar = w.wbar;
-  g.gpos = w.gpos; g.rowsum = w.rowsum; g.pl = w.pl; g.nl = w.nl; g.stat_m = w.stat_m; g.stat_k = w.stat_k;
-  g.dumpS = P ? dumpS : nullptr; g.dumpV = dumpV;
-  g.cstat_m = w.stat_m; g.cstat_k = w.stat_k;
-  g.Xhi = Xh; g.Xlo = Xl;
-  // one GPU: the negatives' own rows come straight from the table (exact fp32, one load); sharded tables would make
-  // that a remote read per row, so they use the local hi + lo slabs
-  if (!P && ent && ent->n_shards == 1 && neg_ids) { g.xids = neg_ids; g.xtab = *ent; }
-  if (!P && w.BnRaw) g.xraw = w.BnRaw;
-  g.gsn = w.gsn;
-  g.out = P ? w.GA : w.Bn;
-  // GEMM2 contracts over the rows of Y: its operand is the transposed slab copy of Y
-  const float *YhT = P ? w.BhiT : w.AhiT, *YlT = P ? w.BloT : w.AloT;
-  const long long rowsX = (long long)p.C * g.Rx * g.nblkD, rowsY = (long long)p.C * g.Ry * g.nblkD;
-  const long long rowsYT = (long long)p.C * slab_blocks(g.Ry) * g.D;
-  CUtensorMap m[6];
-  if (tc_make_map(&m[0], Xh, rowsX, 32, kTileM) || tc_make_map(&m[1], Xl, rowsX, 32, kTileM) ||
-      tc_make_map(&m[2], Yh, rowsY, 32, g.N1) || tc_make_map(&m[3], Yl, rowsY, 32, g.N1) ||
-      tc_make_map(&m[4], YhT, rowsYT, 32, kWc) || tc_make_map(&m[5], YlT, rowsYT, 32, kWc))
-    return KGE_ERR_CUDA;
+  g.VhiT = w.VhiT; g.VloT = w.VloT; g.colpart = w.colpart; g.ncolpart = (p.Cs + kTileM - 1) / kTileM;
+  g.dumpV = dumpV;
   const size_t smem = kRingBytes + 1024;
   const int mtiles = (g.Rx + kTileM - 1) / kTileM;
   int grid = p.C * mtiles;
   if (grid > c.num_sms) grid = c.num_sms;
-  return P ? launch_width<F_P>(c, grid, smem, m, g) : launch_width<F_N>(c, grid, smem, m, g);
+  CUtensorMap m[6];
+  if (P) {
+    g.x2 = w.a2; g.y2 = w.b2;
+    g.pos = w.pos; g.wt = wt; g.wbar = w.wbar;
+    g.gpos = w.gpos; g.rowsum = w.rowsum; g.pl = w.pl; g.nl = w.nl;
+    g.dumpS = dumpS;
+    g.out = w.GA;
+    // GEMM2 contracts over the negatives: its operand is the transposed slab copy of Bn
+    const long long rowsX = (long long)p.C * p.Cs * g.nblkD, rowsY = (long long)p.C * p.Ns * g.nblkD;
+    const long long rowsYT = (long long)p.C * slab_blocks(p.Ns) * p.D;
+    if (tc_make_map(&m[0], w.Ahi, rowsX, 32, kTileM) || tc_make_map(&m[1], w.Alo, rowsX, 32, kTileM) ||
+        tc_make_map(&m[2], w.Bhi, rowsY, 32, g.N1) || tc_make_map(&m[3], w.Blo, rowsY, 32, g.N1) ||
+        tc_make_map(&m[4], w.BhiT, rowsYT, 32, kWc) || tc_make_map(&m[5], w.BloT, rowsYT, 32, kWc))
+      return KGE_ERR_CUDA;
+    return launch_width(c, true, grid, smem, m, g);
+  }
+  g.Xhi = w.Bhi; g.Xlo = w.Blo;
+  // one GPU: the negatives' own rows come straight from the table (exact fp32, one load); sharded tables would make
+  // that a remote read per row, so they use the local hi + lo slabs
+  if (ent && ent->n_shards == 1 && neg_ids) { g.xids = neg_ids; g.xtab = *ent; }
+  if (w.BnRaw) g.xraw = w.BnRaw;
+  g.gsn = w.gsn;
+  g.out = w.Bn;
+  // A operand: V^T slabs [C][Cs/32][Ns][32]; B operand: A^T slabs [C][Cs/32][D][32]; K = i
+  const long long rowsV = (long long)p.C * slab_blocks(p.Cs) * p.Ns, rowsA = (long long)p.C * slab_blocks(p.Cs) * p.D;
+  if (tc_make_map(&m[0], w.VhiT, rowsV, 32, kTileM) || tc_make_map(&m[1], w.VloT, rowsV, 32, kTileM) ||
+      tc_make_map(&m[2], w.AhiT, rowsA, 32, g.N1) || tc_make_map(&m[3], w.AloT, rowsA, 32, g.N1))
+    return KGE_ERR_CUDA;
+  return launch_width(c, false, grid, smem, m, g);
 }
 
 }  // namespace kge
