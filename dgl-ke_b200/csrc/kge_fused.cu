@@ -515,9 +515,14 @@ __device__ __forceinline__ void neg_kblock(float (&acc)[NW / 2], uint64_t dVh, u
   wgmma_commit();
 }
 
+// float2 loads of b in flight per thread in the k_fused<N> chunk epilogue (32 registers next to the accumulator)
+constexpr int kNegEpiLoads = 16;
+
 // G_neg[c][j, d0 : d0 + NW] = sum_i V^T[j, i] A[i, d0 : d0 + NW] for one 128-row tile of negatives j and one output
 // chunk of NW columns per pass over K = Cs; the stages carry the tile's V^T k-block and the chunk's A^T k-block.
-template <int NW>
+// FLAT: the epilogue reads each negative's b as one fp32 row (the table, or the rows the previous step staged);
+// otherwise as hi + lo from the slabs.  The source is fixed per launch, so the column loop never branches on it.
+template <int NW, bool FLAT>
 __global__ void __launch_bounds__(kThreadsF, 1)
 k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUtensorMap mVl,
             const __grid_constant__ CUtensorMap mAh, const __grid_constant__ CUtensorMap mAl, FusedArgs g) {
@@ -604,6 +609,44 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
           for (int t = 0; t < g.ncolpart; ++t) cs[h] += p[(long long)t * g.C * g.Rx];
         }
       }
+      // where this thread's two rows of b start: the row itself (FLAT) or its offset in the slabs, once per tile.  Nothing
+      // writes these sources while the kernel runs (the prefetch warps stage into the other of two buffers), so they are
+      // read through the non-coherent path.
+      bool rok[2];
+      const float* brow[2] = {nullptr, nullptr};
+      long long boff[2] = {0, 0};
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + rloc + 8 * h;
+        rok[h] = m < g.Rx;
+        if (!rok[h]) continue;
+        const long long gx = (long long)c * g.Rx + m;
+        if (FLAT) brow[h] = g.xraw ? g.xraw + gx * (long long)g.D : row_ptr(g.xtab, g.xids[gx]);
+        else boff[h] = slab_off(c, g.nblkD, g.Rx, m, 0);
+      }
+      const long long blk = 32ll * g.Rx;          // slab stride between 32-column blocks of a row
+      // b of column pairs j0 .. j0 + NB - 1 of row h into registers, all of them before any store of the batch: a row
+      // waits for at most ceil(NJ / NB) load round trips per chunk instead of one per column pair
+      constexpr int NJ = NW / 8;                  // column pairs per row and chunk
+      constexpr int NB = FLAT ? kNegEpiLoads : kNegEpiLoads / 2;
+      // the first batch of row 0 goes out before the last k-block's MMAs retire, except on the 256-wide slab path, where
+      // holding it next to the 128-register accumulator makes ptxas spill
+      constexpr bool early = FLAT || NW < 256;
+      float2 bh[NB], bl[NB];
+      auto load_b = [&](int h, int d0, int j0) {
+#pragma unroll
+        for (int jj = 0; jj < NB; ++jj) {
+          const int k = d0 + 8 * (j0 + jj) + 2 * q;
+          if (j0 + jj >= NJ || k >= g.D || !rok[h]) continue;
+          if (FLAT) {
+            bh[jj] = __ldg(reinterpret_cast<const float2*>(brow[h] + k));
+          } else {
+            const long long so = boff[h] + (k >> 5) * blk + (k & 31);
+            bh[jj] = __ldg(reinterpret_cast<const float2*>(g.Xhi + so));
+            bl[jj] = __ldg(reinterpret_cast<const float2*>(g.Xlo + so));
+          }
+        }
+      };
       float gsq[2] = {0.f, 0.f};
       for (int ch = 0; ch < nch; ++ch) {
         const int d0 = ch * NW;
@@ -632,34 +675,31 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
             if (lane == 0) mbar_arrive(&empty[(n - 1) % g.nS1]);
           }
         }
+        if (early) load_b(0, d0, 0);
         wgmma_wait<0>();
         if (lane == 0) mbar_arrive(&empty[(n - 1) % g.nS1]);
         reg_fence(acc);
         // chunk epilogue from the fragment (the producer is already filling the next chunk's stages)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int m = m0 + rloc + 8 * h;
-          if (m >= g.Rx) continue;
-          const long long gx = (long long)c * g.Rx + m;
-          float* orow = g.out + gx * (long long)g.D;
-          const float* brow = g.xraw ? g.xraw + gx * (long long)g.D : (g.xids ? row_ptr(g.xtab, g.xids[gx]) : nullptr);
+          if (!rok[h]) continue;
+          float* orow = g.out + ((long long)c * g.Rx + m0 + rloc + 8 * h) * (long long)g.D;
 #pragma unroll
-          for (int j = 0; j < NW / 8; ++j) {
-            const int k = d0 + 8 * j + 2 * q;
-            if (k >= g.D) continue;
-            float o0 = acc[4 * j + 2 * h], o1 = acc[4 * j + 2 * h + 1];
-            float2 b;
-            if (brow) b = *reinterpret_cast<const float2*>(brow + k);
-            else {
-              const long long so = slab_off(c, g.nblkD, g.Rx, m, k);
-              const float2 bh = *reinterpret_cast<const float2*>(g.Xhi + so), bl = *reinterpret_cast<const float2*>(g.Xlo + so);
-              b = make_float2(bh.x + bl.x, bh.y + bl.y);
+          for (int j0 = 0; j0 < NJ; j0 += NB) {
+            if (!early || h > 0 || j0 > 0) load_b(h, d0, j0);
+#pragma unroll
+            for (int jj = 0; jj < NB; ++jj) {
+              const int j = j0 + jj;
+              const int k = d0 + 8 * j + 2 * q;
+              if (j >= NJ || k >= g.D) continue;
+              float o0 = acc[4 * j + 2 * h], o1 = acc[4 * j + 2 * h + 1];
+              const float2 b = FLAT ? bh[jj] : make_float2(bh[jj].x + bl[jj].x, bh[jj].y + bl[jj].y);
+              if (l2) { o0 = fmaf(b.x, -cs[h], o0); o1 = fmaf(b.y, -cs[h], o1); }   // sum_i V_ij a_i - (sum_i V_ij) b_j
+              o0 += reg_grad_fast(b.x, g.reg_norm, g.reg_coef);
+              o1 += reg_grad_fast(b.y, g.reg_norm, g.reg_coef);
+              gsq[h] += o0 * o0 + o1 * o1;
+              *reinterpret_cast<float2*>(orow + k) = make_float2(o0, o1);
             }
-            if (l2) { o0 = fmaf(b.x, -cs[h], o0); o1 = fmaf(b.y, -cs[h], o1); }   // sum_i V_ij a_i - (sum_i V_ij) b_j
-            o0 += reg_grad_fast(b.x, g.reg_norm, g.reg_coef);
-            o1 += reg_grad_fast(b.y, g.reg_norm, g.reg_coef);
-            gsq[h] += o0 * o0 + o1 * o1;
-            *reinterpret_cast<float2*>(orow + k) = make_float2(o0, o1);
           }
         }
       }
@@ -693,7 +733,8 @@ struct Geometry { int Rx, Ry, N1, nS1, nS2, pf_slots; uint32_t stage1Bytes, stag
 // k_fused<N>: the output-column chunk NW.  A pass over K streams the tile's V^T (128 rows) and the chunk's A^T (NW rows),
 // 128 B per row and k-block, so a CTA streams nch * (128 + NW) rows per k-block for nch = ceil(D / NW) chunks: the
 // width with the fewest is taken (d = 400: 2 x 200 -> 656 rows, against 768 for 2 x 256 and 1024 for 4 x 128).  A
-// 256-wide stage (96 KB) fills the ring twice over, so it is not offered when prefetch slots are wanted.
+// 256-wide stage (96 KB) fills the ring twice over, so it is not offered when prefetch slots are wanted.  Rows streamed
+// decide, not ring depth: at d = 400, 2 stages of 2 x 200 beat 3 stages of 4 x 128 by 15 us per step on an H100.
 int neg_chunk_width(int D, bool want_prefetch) {
   static const int widths[] = {64, 128, 200, 256};
   int best = 0;
@@ -761,11 +802,15 @@ int launch_pos(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, 
                    m[0], m[1], m[2], m[3], m[4], m[5], g);
   return launch_error();
 }
+template <int NW, bool FLAT>
+int launch_neg_src(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+  if (int rc = smem_optin((const void*)k_fused_neg<NW, FLAT>, smem)) return rc;
+  KGE_LAUNCH_NAMED(c, "k_fused<N: G_neg=V^T.A, mean sq>", (k_fused_neg<NW, FLAT>), grid, kThreadsF, smem, m[0], m[1], m[2], m[3], g);
+  return launch_error();
+}
 template <int NW>
 int launch_neg(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
-  if (int rc = smem_optin((const void*)k_fused_neg<NW>, smem)) return rc;
-  KGE_LAUNCH_NAMED(c, "k_fused<N: G_neg=V^T.A, mean sq>", (k_fused_neg<NW>), grid, kThreadsF, smem, m[0], m[1], m[2], m[3], g);
-  return launch_error();
+  return (g.xraw || g.xids) ? launch_neg_src<NW, true>(c, grid, smem, m, g) : launch_neg_src<NW, false>(c, grid, smem, m, g);
 }
 int launch_width(const LaunchCtx& c, bool P, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
   switch (g.N1) {
