@@ -2,12 +2,12 @@
 //
 //   k_fused<P>  rows = positives i, columns = negatives j:
 //               S = A.Bn^T (tensor cores, accumulator in registers) -> loss / self-adversarial softmax / backward
-//               coefficients V computed in place in the accumulator registers -> GA = V.Bn (tensor cores, V as the
-//               REGISTER A operand of wgmma, split into TF32 hi/lo per k-step) -> epilogue.
+//               coefficients V, written to shared memory in the order of wgmma's register A fragment -> GA = V.Bn
+//               (tensor cores, V loaded per k-step as the REGISTER A operand, split into TF32 hi/lo) -> epilogue.
 //               Replaces create_neg (score_fun.py:91-108,268-286,345-376,427-449), LossGenerator.get_total_loss
 //               (loss.py:69-98) and the dL/da half of loss.backward().  The score matrix S never leaves the SM; V leaves
 //               it once, as the transposed TF32 hi/lo slabs V^T[c][i / 32][j][i % 32] plus per-tile column sums
-//               sum_i V_ij, for k_fused<N>.
+//               sum_i V_ij, for k_fused<N>; spare warps write both from the shared-memory copy while GEMM2 runs.
 //   k_fused<N>  rows = negatives j:  G_neg = V^T.A - colsum*b + reg'(b), mean(G_neg^2)  (the dL/db half of
 //               loss.backward() plus phase 1 of ExternalEmbedding.update for the negatives, tensor_models.py:316-328).
 //               One pipelined GEMM over K = Cs with both operands from shared memory: V^T slabs (written by k_fused<P>)
@@ -20,14 +20,16 @@
 // matrix take its transposed slabs (kge_common.cuh:slabT_off).
 //
 // CTA = 384 threads: warpgroups 0 and 1 (warps 0-7) each own 64 rows of the 128-row tile -- MMA issue and epilogue on
-// the accumulator fragment, a row lives in the 4 lanes of a quad; warp 8 TMA producer, warp 9 idle (setmaxnreg acts on
-// whole warpgroups), warps 10-11 prefetch the next step's rows.  Persistent over (chunk, 128-row tile) work items.
-// Shared memory: one 192 KB ring.  k_fused<P> uses it as nS1 stages {X_hi,X_lo,Y_hi,Y_lo} for GEMM1 and as nS2 stages
-// {Y^T_hi,Y^T_lo} for GEMM2, whose output is produced in 128-column chunks; k_fused<N> as nS stages
-// {V^T_hi,V^T_lo,A^T_hi,A^T_lo} of one output-column chunk of width NW.
+// the accumulator fragment, a row lives in the 4 lanes of a quad; warp 8 TMA producer, warps 10-11 prefetch the next
+// step's rows; in k_fused<P> warp 9 (and 10-11 when they do not prefetch) write the V hand-off.  Persistent over
+// (chunk, 128-row tile) work items.
+// Shared memory: one ring.  k_fused<P> (223 KB, 192 KB with prefetch slots) uses it as nS1 stages {X_hi,X_lo,Y_hi,Y_lo} for GEMM1, then as
+// the V buffer followed by nS2 stages {Y^T_hi,Y^T_lo} for GEMM2, whose output is produced in chunks of NW columns;
+// k_fused<N> (192 KB) as nS stages {V^T_hi,V^T_lo,A^T_hi,A^T_lo} of one output-column chunk of width NW.
 #include <cuda.h>
 #include <cstdio>
 #include <cstdlib>
+#include <mutex>
 #include "kge_common.cuh"
 #include "kge_tc.cuh"
 
@@ -40,10 +42,13 @@ namespace {
 constexpr int kTileM = 128;
 constexpr int kThreadsF = 384;                    // warps 0-7 MMA + epilogue (two warpgroups), 8 TMA producer, 10-11 prefetch
 constexpr int kProducerWarp = 8;
+constexpr int kHandoffWarp = 9;                    // k_fused<P>: first of the warps that write the V hand-off
 constexpr int kMaxS1 = 4, kMaxS2 = 8;
 constexpr int kMaxPf = 8;                          // row slots per prefetch warp
-constexpr uint32_t kRingBytes = 192 * 1024;
-constexpr int kWc = 128;                           // k_fused<P> GEMM2 output-column chunk = wgmma N
+constexpr uint32_t kRingBytes = 192 * 1024;        // k_fused<N>
+// k_fused<P>: the 227 KB a CTA may opt in to, less the 1 KB alignment slack of the ring, the kernel's static shared
+// memory (mbarriers, |b|^2 of the chunk, the row scales: 2 KB as ptxas reports it) and 1 KB to spare
+constexpr uint32_t kRingBytesP = 223 * 1024;
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
@@ -54,6 +59,7 @@ struct FusedArgs {
   int reg_norm;
   int C, Rx, Ry, D;      // rows per chunk on the lane side / on the contraction side of the last GEMM, row length
   int N1;                // P: wgmma N of GEMM1 (the kernel variant's width, >= Ry);  N: output-column chunk width
+  int N2;                // P: output-column chunk width of GEMM2
   int nblkD;             // 32-column slab blocks of D
   int nS1, nS2;          // P: GEMM1 / GEMM2 stages;  N: nS1 stages
   uint32_t stage1Bytes, stage2Bytes;
@@ -159,33 +165,99 @@ __device__ __forceinline__ void prefetch_rows(const FusedArgs& g, uint8_t* ring,
   __syncwarp();
 }
 
+// one k-block of a GEMM with both operands in shared memory: KS k-steps of 8, each hi*hi + hi*lo + lo*hi, as one wgmma
+// group.  A guard between the fence and the commit would make ptxas insert warpgroup arrives of its own, so callers
+// switch over the k-step count.
+template <int NW, int KS>
+__device__ __forceinline__ void kblock_3xtf32(float (&acc)[NW / 2], uint64_t dXh, uint64_t dXl, uint64_t dYh, uint64_t dYl) {
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    const uint64_t o = (uint64_t)(ks * 2);     // K-major: +32 bytes per k-step inside the 128-byte swizzle span
+    wgmma_ss<NW>(acc, dXh + o, dYh + o, 1u);
+    wgmma_ss<NW>(acc, dXh + o, dYl + o, 1u);
+    wgmma_ss<NW>(acc, dXl + o, dYh + o, 1u);
+  }
+  wgmma_commit();
+}
+
 // ================================ k_fused<P> ================================
+// The coefficients V of the tile in shared memory, in the order of GEMM2's register A fragment: per MMA warp w and k-step
+// j (8 columns), 32 lanes x 16 bytes = (row, k = q), (row + 8, q), (row, q + 4), (row + 8, q + 4) of lane 4 g + q, so a
+// k-step is one 16-byte ld.shared per thread.  The lane's 16 bytes sit at position L ^ ((L >> 3) & 3): the fragment
+// loads stay conflict-free (the 8 lanes of a quarter warp keep distinct positions mod 8, so they cover all 32 banks);
+// the scalar stores from the accumulator fragment (32 lanes, 16 lane positions) and the hand-off warps' column reads
+// (32 consecutive rows of one column) both reach 16 banks, so every bank at most twice.  Returns the float index.
 template <int NV>
+__device__ __forceinline__ int vsm_idx(int i, int k) {          // i: row of the tile (0..127), k: column (0..NV-1)
+  const int g = i & 7, h = (i >> 3) & 1, kk = k & 7;
+  const int L = 4 * g + (kk & 3);
+  return (((i >> 4) * (NV / 8) + (k >> 3)) * 32 + (L ^ ((L >> 3) & 3))) * 4 + h + 2 * (kk >> 2);
+}
+
+// GEMM2 k-step j of one output chunk: the fragment from shared memory, split into TF32 hi/lo, hi*hi + hi*lo + lo*hi as one
+// wgmma group.  Two fragment sets alternate (a set is re-written only once the group that reads it has retired).
+template <int NW>
+__device__ __forceinline__ void pos_kstep(float (&acc2)[NW / 2], uint32_t (&ah)[4], uint32_t (&al)[4], const float* vf,
+                                          uint64_t dYh, uint64_t dYl) {
+  const float4 v = *reinterpret_cast<const float4*>(vf);
+  const float a[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    float hi, lo;
+    split_tf32(a[r], hi, lo);
+    ah[r] = __float_as_uint(hi); al[r] = __float_as_uint(lo);
+  }
+  wgmma_fence();
+  wgmma_rs<NW>(acc2, ah, dYh, 1u);
+  wgmma_rs<NW>(acc2, ah, dYl, 1u);
+  wgmma_rs<NW>(acc2, al, dYh, 1u);
+  wgmma_commit();
+}
+
+// this thread's first row inside the 128-row tile (16 per warp, lane / 4; the second is 8 further): read from %tid.x
+// where it is needed rather than held across GEMM1 and the softmax passes, where every register not taken by the score
+// accumulator is wanted and ptxas would spill it
+__device__ __forceinline__ int tile_row() {
+  uint32_t t;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+  return (int)((t >> 5) * 16 + ((t >> 2) & 7));
+}
+
+template <int NV, int NW>
 __global__ void __launch_bounds__(kThreadsF, 1)
 k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtensorMap mXl,
             const __grid_constant__ CUtensorMap mYh1, const __grid_constant__ CUtensorMap mYl1,
             const __grid_constant__ CUtensorMap mYh2, const __grid_constant__ CUtensorMap mYl2, FusedArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full1[kMaxS1], empty1[kMaxS1], full2[kMaxS2], empty2[kMaxS2];
+  __shared__ __align__(8) uint64_t vfree;           // the tile's V buffer is no longer read (MMA and hand-off warps)
   __shared__ __align__(8) uint64_t pf_full[2][kMaxPf];
   __shared__ __align__(16) float colA[NV];
-  __shared__ __align__(16) float cpart[8][NV];     // column sums of V over the 16 rows of each MMA warp
+  __shared__ float rsc[kTileM];                    // 1 / softmax denominator (or 1 / Ns) of each row of the tile
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint8_t* ring = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  float* vsm = reinterpret_cast<float*>(ring);      // V buffer: overlays the GEMM1 stages, ahead of the GEMM2 stages
+  constexpr uint32_t vBytes = (uint32_t)NV * 512u;  // 8 warps x NV / 8 k-steps x 512 bytes
+  uint8_t* ring2 = ring + vBytes;
 
   const int mtiles = (g.Rx + kTileM - 1) / kTileM;
   const int ntiles = g.C * mtiles;
   const int nkb1 = (g.D + 31) >> 5;
   const int nkb2 = (g.Ry + 31) >> 5;
-  const int nchunks = (g.D + kWc - 1) / kWc;
+  const int nchunks = (g.D + NW - 1) / NW;
   constexpr uint32_t yBytes1 = (uint32_t)NV * 128u;
-  constexpr uint32_t yBytes2 = (uint32_t)kWc * 128u;
+  constexpr uint32_t yBytes2 = (uint32_t)NW * 128u;
   const bool l2 = g.model == KGE_TRANSE_L2;
+  // the hand-off warps: warp 9, and warps 10-11 when they do not prefetch; they meet the MMA warps at named barrier 2
+  const int nhand = g.pf_slots > 0 ? 1 : 3;
+  const uint32_t hand_bar_n = 256u + 32u * (uint32_t)nhand;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kMaxS1; ++s) { mbar_init(&full1[s], 1); mbar_init(&empty1[s], 8); }
     for (int s = 0; s < kMaxS2; ++s) { mbar_init(&full2[s], 1); mbar_init(&empty2[s], 8); }
+    mbar_init(&vfree, 8 + nhand);
     for (int s = 0; s < kMaxPf; ++s) { mbar_init(&pf_full[0][s], 1); mbar_init(&pf_full[1][s], 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -196,17 +268,18 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
   __syncthreads();
 
   // Roles.  The producer runs its loop with all 32 lanes (warp-uniform control flow) and one elected lane issues the
-  // TMA ops.  Registers: the third warpgroup (producer, prefetch warps) hands most of its share to the two MMA
-  // warpgroups, which keep the score accumulator and a GEMM2 accumulator chunk in registers.
+  // TMA ops.  Registers: the third warpgroup (producer, hand-off and prefetch warps) hands most of its share to the two
+  // MMA warpgroups, which keep the score accumulator and then a GEMM2 accumulator chunk in registers.
   if (warp >= 8) {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
   if (warp == kProducerWarp) {
     // ================================ TMA producer ================================
-    uint32_t n1 = 0, n2 = 0;      // stage fills issued so far (GEMM1 / GEMM2)
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    uint32_t n1 = 0, n2 = 0, it = 0;   // stage fills issued so far (GEMM1 / GEMM2), tiles so far
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
       const int c = tile / mtiles, m0 = (tile % mtiles) * kTileM;
-      // the ring is about to be re-used with the GEMM1 layout: every GEMM2 stage of the previous tile must be consumed
-      for (uint32_t k = (n2 > (uint32_t)g.nS2 ? n2 - g.nS2 : 0); k < n2; ++k) mbar_wait(&empty2[k % g.nS2], (k / g.nS2) & 1);
+      // the ring is about to be re-used with the GEMM1 layout: the previous tile's GEMM2 stages are consumed and its V
+      // buffer is read (every MMA warp has retired its last GEMM2 group, every hand-off warp is done)
+      if (it > 0) mbar_wait(&vfree, (it - 1) & 1);
       for (int kb = 0; kb < nkb1; ++kb, ++n1) {
         const uint32_t s = n1 % g.nS1;
         mbar_wait(&empty1[s], ((n1 / g.nS1) & 1) ^ 1);
@@ -229,9 +302,9 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
         for (int kb = 0; kb < nkb2; ++kb, ++n2) {
           const uint32_t s = n2 % g.nS2;
           mbar_wait(&empty2[s], ((n2 / g.nS2) & 1) ^ 1);
-          uint8_t* st = ring + (size_t)s * g.stage2Bytes;
+          uint8_t* st = ring2 + (size_t)s * g.stage2Bytes;
           // transposed slabs: TMA row of (chunk c, 32-row block kb of Y, column d) = (c * nblkRy + kb) * D + d
-          const int yy = (c * nkb2 + kb) * g.D + ch * kWc;
+          const int yy = (c * nkb2 + kb) * g.D + ch * NW;
           if (elect_one()) {
             mbar_expect_tx(&full2[s], 2u * yBytes2);
             tma_load_2d(st, &mYh2, &full2[s], 0, yy);
@@ -241,6 +314,48 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
         }
       }
     }
+  } else if (warp - kHandoffWarp < nhand) {
+    // ================================ V hand-off to k_fused<N> ================================
+    // V_ij = coef_ij / den_i as TF32 hi/lo in the transposed slabs V^T[c][i / 32][j][i % 32]: per column j and 32-row
+    // block, one lane per row, so every store is a whole 128-byte line; rows i >= Cs are not written (k_fused<N> never
+    // reads them).  TransE_l2 also needs sum_i V_ij over the tile: each lane adds its rows of the blocks in order, then
+    // a fixed butterfly over the lanes.  Both are read from the shared-memory copy while the MMA warps run GEMM2.
+    const int hw = warp - kHandoffWarp;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      const int c = tile / mtiles, m0 = (tile % mtiles) * kTileM;
+      const int rows = g.Rx - m0 < kTileM ? g.Rx - m0 : kTileM;
+      const int nb = (rows + 31) >> 5;
+      asm volatile("bar.sync 2, %0;" ::"r"(hand_bar_n) : "memory");     // V and rsc of the tile are in shared memory
+      float* dst = g.colpart + (long long)(tile % mtiles) * g.C * g.Ry + (long long)c * g.Ry;
+      for (int j = hw; j < g.Ry; j += nhand) {
+        float s = 0.f;
+        float v[kTileM / 32];                      // all blocks' loads issued before the first store
+#pragma unroll
+        for (int b = 0; b < kTileM / 32; ++b) {
+          const int i = 32 * b + lane;
+          v[b] = b < nb ? vsm[vsm_idx<NV>(i, j)] * rsc[i] : 0.f;
+        }
+#pragma unroll
+        for (int b = 0; b < kTileM / 32; ++b) {
+          const int i = 32 * b + lane;
+          if (i < rows) {
+            float hi, lo;
+            split_tf32(v[b], hi, lo);
+            const long long o = slabT_off(c, g.Rx, g.Ry, m0 + i, j);
+            g.VhiT[o] = hi; g.VloT[o] = lo;
+          }
+          s += v[b];
+        }
+        if (l2) {
+#pragma unroll
+          for (int x = 16; x >= 1; x >>= 1) s += __shfl_xor_sync(0xffffffffu, s, x);
+          if (lane == 0) dst[j] = s;
+        }
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the next tile's TMA writes over the buffer
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&vfree);
+    }
   } else if (warp >= 10 && g.pf_slots > 0) {
     prefetch_rows(g, ring, pf_full, warp - 10, lane);
   }
@@ -249,9 +364,7 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
     asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
     const int wg = warp >> 2, q = lane & 3;
     const int et = threadIdx.x;                   // 0..255
-    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread's rows inside the tile: rloc, rloc + 8
     uint32_t n1 = 0, n2 = 0;
-    float acc[NV / 2];                            // S -> V: rows rloc (+8), columns 8 j + 2 q + {0, 1}
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const int c = tile / mtiles, m0 = (tile % mtiles) * kTileM;
       epi_bar();                                  // everybody is done with the previous tile's shared constants
@@ -260,6 +373,9 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
         colA[y] = (l2 && ok) ? g.y2[(long long)c * g.Ry + y] : 0.f;
       }
       epi_bar();
+      float rscal[2];                             // 1 / softmax denominator (or 1 / Ns) of the two rows
+      {
+      float acc[NV / 2];                          // S -> V: rows rloc (+8), columns 8 j + 2 q + {0, 1}
       // ---- GEMM1: S = X . Y^T, K = D ----
 #pragma unroll
       for (int i = 0; i < NV / 2; ++i) acc[i] = 0.f;
@@ -271,14 +387,13 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
         const uint64_t dYh = make_desc(st + 32768u), dYl = make_desc(st + 32768u + yBytes1);
         const int kleft = g.D - kb * 32;
         const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
-        wgmma_fence();
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const uint64_t o = (uint64_t)(ks * 2);     // K-major: +32 bytes per k-step inside the 128-byte swizzle span
-          wgmma_ss<NV>(acc, dXh + o, dYh + o, 1u);
-          wgmma_ss<NV>(acc, dXh + o, dYl + o, 1u);
-          wgmma_ss<NV>(acc, dXl + o, dYh + o, 1u);
+        // one straight-line fence .. wgmma .. commit sequence per k-step count (see neg_kblock)
+        switch (ksteps) {
+          case 4: kblock_3xtf32<NV, 4>(acc, dXh, dXl, dYh, dYl); break;
+          case 3: kblock_3xtf32<NV, 3>(acc, dXh, dXl, dYh, dYl); break;
+          case 2: kblock_3xtf32<NV, 2>(acc, dXh, dXl, dYh, dYl); break;
+          default: kblock_3xtf32<NV, 1>(acc, dXh, dXl, dYh, dYl); break;
         }
-        wgmma_commit();
         if (kb > 0) {
           wgmma_wait<1>();                           // the previous k-block has retired: its stage is free
           if (lane == 0) mbar_arrive(&empty1[(n1 - 1) % g.nS1]);
@@ -287,9 +402,10 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(&empty1[(n1 - 1) % g.nS1]);
       reg_fence(acc);
+      epi_bar();                                  // both warpgroups' GEMM1 has retired: the V buffer may overwrite the stages
+      const int rloc = tile_row();                // this thread's rows inside the tile: rloc, rloc + 8
 
-      // ---- S -> V in place, two rows per thread; a row's statistics are reduced over the 4 lanes of its quad ----
-      float rscal[2];                             // 1 / softmax denominator (or 1 / Ns) of the two rows
+      // ---- S -> V, two rows per thread; a row's statistics are reduced over the 4 lanes of its quad ----
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int m = m0 + rloc + 8 * h;
@@ -326,9 +442,9 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
         } else {
           mxl = 0.f;
         }
-        // ---- pass C: softmax numerators, loss terms and (unnormalised) backward coefficients.  The 1/denominator of
-        //      the row is a per-row scalar: it is applied to the loss sums here and to the row of GA in the GEMM2
-        //      epilogue. ----
+        // ---- pass C: softmax numerators, loss terms and (unnormalised) backward coefficients, which go to the V
+        //      buffer.  The 1/denominator of the row is a per-row scalar: it is applied to the loss sums here, to the
+        //      hand-off by the hand-off warps and to the row of GA in the GEMM2 epilogue. ----
         float nls = 0.f, rs = 0.f, den = 0.f;
 #pragma unroll
         for (int j = 0; j < NV / 8; ++j) {
@@ -353,7 +469,7 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
             const float coef = ok ? pe * sig * kw * rinv : 0.f;              // dL/dneg_ij (/ dist) * denominator
             if (ok) { nls = fmaf(pe, sp, nls); den += pe; }
             rs += coef;
-            acc[4 * j + 2 * h + e] = coef;
+            vsm[vsm_idx<NV>(rloc + 8 * h, col)] = coef;
           }
         }
         den += __shfl_xor_sync(0xffffffffu, den, 1); den += __shfl_xor_sync(0xffffffffu, den, 2);
@@ -361,41 +477,12 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
         rs += __shfl_xor_sync(0xffffffffu, rs, 1); rs += __shfl_xor_sync(0xffffffffu, rs, 2);
         const float rscale = g.adversarial ? (row_ok ? 1.f / den : 0.f) : g.uni;
         rscal[h] = rscale;
-        if (g.dumpV && row_ok) {        // test hook: the dump shows the normalised coefficients
-#pragma unroll
+        if (g.dumpV && row_ok) {        // test hook: the dump shows the normalised coefficients (each thread's own)
           for (int j = 0; j < NV / 8; ++j)
             if (8 * j + 2 * q < g.Ry)
               *reinterpret_cast<float2*>(g.dumpV + gx * g.Ry + 8 * j + 2 * q) =
-                  make_float2(acc[4 * j + 2 * h] * rscale, acc[4 * j + 2 * h + 1] * rscale);
-        }
-        // ---- hand V to k_fused<N>: V_ij = coef_ij / den_i as TF32 hi/lo in the transposed slabs
-        //      V^T[c][i / 32][j][i % 32].  The 8 lanes that share q hold 8 consecutive i of the same j, so every store
-        //      fills a whole 32-byte sector; rows i >= Cs and columns j >= Ns are not written (k_fused<N> never reads
-        //      them).  TransE_l2 also needs sum_i V_ij: summed over the 16 rows of the warp by shuffles and the two
-        //      rows of the thread in cpart, then over the 8 warps after the loop. ----
-        {
-          float* vh = g.VhiT + slabT_off(c, g.Rx, g.Ry, m, 0);
-          float* vl = g.VloT + slabT_off(c, g.Rx, g.Ry, m, 0);
-#pragma unroll
-          for (int j = 0; j < NV / 8; ++j) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int col = 8 * j + 2 * q + e;
-              const float v = acc[4 * j + 2 * h + e] * rscale;
-              if (row_ok && col < g.Ry) {
-                float hi, lo;
-                split_tf32(v, hi, lo);
-                vh[col * 32] = hi; vl[col * 32] = lo;
-              }
-              if (l2) {
-                float s = v;
-                s += __shfl_xor_sync(0xffffffffu, s, 4);
-                s += __shfl_xor_sync(0xffffffffu, s, 8);
-                s += __shfl_xor_sync(0xffffffffu, s, 16);
-                if (lane < 4) cpart[warp][col] = h ? cpart[warp][col] + s : s;
-              }
-            }
-          }
+                  make_float2(vsm[vsm_idx<NV>(rloc + 8 * h, 8 * j + 2 * q)] * rscale,
+                              vsm[vsm_idx<NV>(rloc + 8 * h, 8 * j + 2 * q + 1)] * rscale);
         }
         if (q == 0 && row_ok) {
           const float ps = g.pos[gx];
@@ -406,80 +493,49 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
           if (l2) g.rowsum[gx] = rs * rscale;
         }
       }
-      if (l2) {
-        epi_bar();                                // every warp's column sums are in cpart
-        float* dst = g.colpart + (long long)(tile % mtiles) * g.C * g.Ry + (long long)c * g.Ry;
-        for (int y = et; y < g.Ry; y += 256) {
-          float s = cpart[0][y];
-#pragma unroll
-          for (int w = 1; w < 8; ++w) s += cpart[w][y];
-          dst[y] = s;
-        }
+      if (q == 0) { rsc[rloc] = rscal[0]; rsc[rloc + 8] = rscal[1]; }
       }
-      // ---- accumulator fragment -> register A fragment of GEMM2: within every group of 8 columns a thread holds columns
-      //      2q, 2q+1 and wgmma wants k = q, q + 4 from it: exchange inside the quad.  Afterwards acc[4 j + 0..3] =
-      //      (row, k = q), (row + 8, q), (row, q + 4), (row + 8, q + 4) of k-step j. ----
-      {
-        const int srcLo = (lane & ~3) | (q >> 1), srcHi = srcLo + 2;
-        const bool odd = q & 1;
-#pragma unroll
-        for (int j = 0; j < NV / 8; ++j) {
-          float o[4];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-            const float a0 = __shfl_sync(0xffffffffu, v0, srcLo), a1 = __shfl_sync(0xffffffffu, v1, srcLo);
-            const float b0 = __shfl_sync(0xffffffffu, v0, srcHi), b1 = __shfl_sync(0xffffffffu, v1, srcHi);
-            o[h] = odd ? a1 : a0;
-            o[2 + h] = odd ? b1 : b0;
-          }
-          acc[4 * j + 0] = o[0]; acc[4 * j + 1] = o[1]; acc[4 * j + 2] = o[2]; acc[4 * j + 3] = o[3];
-        }
-      }
+      // the hand-off warps may read the tile's V and row scales; this warp reads back only its own rows
+      asm volatile("bar.arrive 2, %0;" ::"r"(hand_bar_n) : "memory");
+      __syncwarp();
 
-      // ---- GEMM2: GA[:, chunk] = V . Bn[:, chunk], K = Ns, A operand from registers; epilogue per 128-column chunk ----
+      // ---- GEMM2: GA[:, chunk] = V . Bn[:, chunk], K = Ns, A operand from the V buffer; epilogue per NW-column chunk.
+      //      One wgmma group per k-step, at most two in flight: a stage is released once the group of the next
+      //      k-block's first k-step has been issued and its own last group has retired. ----
+      const float* vw = vsm + ((warp * (NV / 8)) * 32 + (lane ^ ((lane >> 3) & 3))) * 4;
+      const int rloc = tile_row();
       for (int ch = 0; ch < nchunks; ++ch) {
-        const int d0 = ch * kWc;
-        float acc2[kWc / 2];
+        const int d0 = ch * NW;
+        float acc2[NW / 2];
 #pragma unroll
-        for (int i = 0; i < kWc / 2; ++i) acc2[i] = 0.f;
-#pragma unroll
-        for (int kb = 0; kb < (NV + 31) / 32; ++kb) {
-          if (kb >= nkb2) break;
+        for (int i = 0; i < NW / 2; ++i) acc2[i] = 0.f;
+        uint32_t ah[2][4], al[2][4];
+#pragma unroll 1
+        for (int kb = 0; kb < nkb2; ++kb) {
           const uint32_t s = n2 % g.nS2;
           mbar_wait(&full2[s], (n2 / g.nS2) & 1);
-          const uint32_t st = smem_u32(ring + (size_t)s * g.stage2Bytes);
+          const uint32_t st = smem_u32(ring2 + (size_t)s * g.stage2Bytes);
           const uint64_t dYh = make_desc(st), dYl = make_desc(st + yBytes2);
           const int kleft = g.Ry - kb * 32;
           const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
-          // the register operands of an in-flight wgmma must stay untouched: two sets, alternating, one k-step in flight
-          // behind the one being prepared
-          uint32_t ah[2][4] = {}, al[2][4] = {};
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) {
-            const int j = kb * 4 + ks;                  // compile-time: both loops are unrolled
-            if (j < NV / 8 && ks < ksteps) {
-              if (ks >= 2) wgmma_wait<1>();
-#pragma unroll
-              for (int r = 0; r < 4; ++r) {
-                float hi, lo;
-                split_tf32(acc[4 * j + r], hi, lo);
-                ah[ks & 1][r] = __float_as_uint(hi); al[ks & 1][r] = __float_as_uint(lo);
-              }
-              wgmma_fence();
+            const int j = kb * 4 + ks;
+            if (ks < ksteps) {
               const uint64_t o = (uint64_t)(ks * 2);
-              wgmma_rs<kWc>(acc2, ah[ks & 1], dYh + o, 1u);
-              wgmma_rs<kWc>(acc2, ah[ks & 1], dYl + o, 1u);
-              wgmma_rs<kWc>(acc2, al[ks & 1], dYh + o, 1u);
-              wgmma_commit();
-              if (ks >= 1) { reg_fence(ah[(ks - 1) & 1]); reg_fence(al[(ks - 1) & 1]); }
+              pos_kstep<NW>(acc2, ah[j & 1], al[j & 1], vw + j * 128, dYh + o, dYl + o);
+              if (j > 0) {
+                wgmma_wait<1>();                        // k-step j - 1 has retired: its fragment set is free
+                reg_fence(ah[(j - 1) & 1]); reg_fence(al[(j - 1) & 1]);
+                if (ks == 0 && lane == 0) mbar_arrive(&empty2[(n2 - 1) % g.nS2]);   // ... and so has k-block kb - 1
+              }
             }
           }
-          wgmma_wait<0>();
-          reg_fence(ah[0]); reg_fence(ah[1]); reg_fence(al[0]); reg_fence(al[1]);
-          if (lane == 0) mbar_arrive(&empty2[s]);
           ++n2;
         }
+        wgmma_wait<0>();
+        reg_fence(ah[0]); reg_fence(ah[1]); reg_fence(al[0]); reg_fence(al[1]);
+        if (lane == 0) mbar_arrive(&empty2[(n2 - 1) % g.nS2]);
         reg_fence(acc2);
         // chunk epilogue from the fragment: rows rloc (+8), columns d0 + 8 j + 2 q + {0, 1}
 #pragma unroll
@@ -488,7 +544,7 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
           if (m >= g.Rx) continue;
           float* orow = g.out + ((long long)c * g.Rx + m) * (long long)g.D;
 #pragma unroll
-          for (int j = 0; j < kWc / 8; ++j) {
+          for (int j = 0; j < NW / 8; ++j) {
             const int k = d0 + 8 * j + 2 * q;
             if (k >= g.D) continue;
             // 1 / softmax denominator of the row
@@ -496,25 +552,14 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
           }
         }
       }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the next tile's TMA writes over the V buffer
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&vfree);
     }
   }
 }
 
 // ================================ k_fused<N> ================================
-// one k-block of G_neg: KS k-steps of 8, each hi*hi + hi*lo + lo*hi, as one wgmma group
-template <int NW, int KS>
-__device__ __forceinline__ void neg_kblock(float (&acc)[NW / 2], uint64_t dVh, uint64_t dVl, uint64_t dAh, uint64_t dAl) {
-  wgmma_fence();
-#pragma unroll
-  for (int ks = 0; ks < KS; ++ks) {
-    const uint64_t o = (uint64_t)(ks * 2);     // K-major: +32 bytes per k-step inside the 128-byte swizzle span
-    wgmma_ss<NW>(acc, dVh + o, dAh + o, 1u);
-    wgmma_ss<NW>(acc, dVh + o, dAl + o, 1u);
-    wgmma_ss<NW>(acc, dVl + o, dAh + o, 1u);
-  }
-  wgmma_commit();
-}
-
 // float2 loads of b in flight per thread in the k_fused<N> chunk epilogue (32 registers next to the accumulator)
 constexpr int kNegEpiLoads = 16;
 
@@ -665,10 +710,10 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
           // one straight-line fence .. wgmma .. commit sequence per k-step count: a guard between the fence and the
           // commit makes ptxas insert warpgroup arrives of its own
           switch (ksteps) {
-            case 4: neg_kblock<NW, 4>(acc, dVh, dVl, dAh, dAl); break;
-            case 3: neg_kblock<NW, 3>(acc, dVh, dVl, dAh, dAl); break;
-            case 2: neg_kblock<NW, 2>(acc, dVh, dVl, dAh, dAl); break;
-            default: neg_kblock<NW, 1>(acc, dVh, dVl, dAh, dAl); break;
+            case 4: kblock_3xtf32<NW, 4>(acc, dVh, dVl, dAh, dAl); break;
+            case 3: kblock_3xtf32<NW, 3>(acc, dVh, dVl, dAh, dAl); break;
+            case 2: kblock_3xtf32<NW, 2>(acc, dVh, dVl, dAh, dAl); break;
+            default: kblock_3xtf32<NW, 1>(acc, dVh, dVl, dAh, dAl); break;
           }
           if (kb > 0) {
             wgmma_wait<1>();                           // the previous k-block has retired: its stage is free
@@ -719,7 +764,7 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
 }  // namespace
 
 // The fused kernel keeps a whole row of the chunk's score matrix in the accumulator registers of one warpgroup
-// (columns / 2 registers per thread, next to the 64 of a GEMM2 chunk): at most 240 columns.
+// (columns / 2 registers per thread): at most 240 columns.
 // Its operands are those of the wgmma engine, and its epilogue is the plain (non-pairwise, unmasked) Logsigmoid criterion.
 bool fused_supported(const StepParams& p) {
   return umma_supported(p) && !p.hinge && !p.pairwise && !p.neg_deg && p.Cs <= 240 && p.Ns <= 240;
@@ -728,7 +773,7 @@ bool fused_supported(const StepParams& p) {
 // mode 0 (P): S = A.Bn^T -> loss, coefficients V -> GA, V^T slabs;  mode 1 (N): G_neg = V^T.A (+ mean square)
 namespace {
 // GEMM stage geometry of one mode + what the ring leaves for prefetch row slots
-struct Geometry { int Rx, Ry, N1, nS1, nS2, pf_slots; uint32_t stage1Bytes, stage2Bytes, pf_off; bool ok; };
+struct Geometry { int Rx, Ry, N1, N2, nS1, nS2, pf_slots; uint32_t ringBytes, stage1Bytes, stage2Bytes, pf_off; bool ok; };
 
 // k_fused<N>: the output-column chunk NW.  A pass over K streams the tile's V^T (128 rows) and the chunk's A^T (NW rows),
 // 128 B per row and k-block, so a CTA streams nch * (128 + NW) rows per k-block for nch = ceil(D / NW) chunks: the
@@ -752,6 +797,7 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
   const uint32_t row = (uint32_t)p.D * 4u;
   if (mode == 1) {
     q.Rx = p.Ns; q.Ry = p.Cs;
+    q.ringBytes = kRingBytes;
     q.N1 = neg_chunk_width(p.D, want_prefetch);
     q.stage1Bytes = 2u * kTileM * 128u + 2u * (uint32_t)q.N1 * 128u;
     q.nS1 = (int)(kRingBytes / q.stage1Bytes); if (q.nS1 > kMaxS1) q.nS1 = kMaxS1;
@@ -770,37 +816,81 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
   q.Rx = p.Cs; q.Ry = p.Ns;
   // wgmma's N is part of the instruction: the kernel is instantiated for these widths
   q.N1 = q.Ry <= 64 ? 64 : (q.Ry <= 128 ? 128 : (q.Ry <= 208 ? 208 : 256));
+  // With prefetch slots the ring keeps the 192 KB they were carved from before the V buffer: whether the next step's
+  // rows can be staged, and in how many slots, does not depend on the GEMM2 layout.  Without them it takes what a CTA
+  // may opt in to.
+  const uint32_t ring = want_prefetch ? kRingBytes : kRingBytesP;
+  q.ringBytes = ring;
   q.stage1Bytes = 2u * 16384u + 2u * (uint32_t)q.N1 * 128u;
-  q.stage2Bytes = 2u * (uint32_t)kWc * 128u;
-  q.nS1 = (int)(kRingBytes / q.stage1Bytes); if (q.nS1 > kMaxS1) q.nS1 = kMaxS1;
-  q.nS2 = (int)(kRingBytes / q.stage2Bytes); if (q.nS2 > kMaxS2) q.nS2 = kMaxS2;
-  q.ok = q.nS1 >= 2 && q.nS2 >= 2;
-  if (q.ok && want_prefetch) {
-    // GEMM1 keeps its stages; GEMM2 gives up stages (never below 4) until both prefetch warps have kMaxPf row slots
-    int nS1 = q.nS1, nS2 = q.nS2;
-    uint32_t want = 2u * kMaxPf * row;
-    while (nS1 > 2 && kRingBytes - (uint32_t)nS1 * q.stage1Bytes < want) --nS1;   // a deep GEMM1 ring gives up stages first
-    uint32_t used = (uint32_t)nS1 * q.stage1Bytes;
-    if (want > kRingBytes - used) want = kRingBytes - used;           // never more than GEMM1 leaves
-    while (nS2 > 4 && kRingBytes - (uint32_t)nS2 * q.stage2Bytes < want) --nS2;
-    if ((uint32_t)nS2 * q.stage2Bytes > used) used = (uint32_t)nS2 * q.stage2Bytes;
-    int slots = (int)((kRingBytes - used) / (2u * row));
+  int nS1 = (int)(ring / q.stage1Bytes); if (nS1 > kMaxS1) nS1 = kMaxS1;
+  if (nS1 < 2) return q;
+  // GEMM2 needs the V buffer (N1 / 8 k-steps x 512 B per MMA warp) ahead of its stages.  Its output-column chunk NW:
+  // a chunk streams NW rows of Bn^T per k-block and issues NW columns of MMAs, so ceil(D / NW) * NW should be least
+  // (d = 400: 2 x 200 = 400 against 4 x 128 = 512; d = 800: 4 x 200 against 7 x 128 = 896), 128 on a tie.  256 never
+  // does better than 128.  A width is taken if the ring holds the buffer and 2 of its stages and, when prefetch slots
+  // are wanted, leaves at least 2 of them; otherwise the next width, and prefetch goes only when neither leaves 2.
+  const uint32_t vBytes = (uint32_t)q.N1 * 512u;
+  const bool w200 = (p.D + 199) / 200 * 200 < (p.D + 127) / 128 * 128;
+  const int widths[2] = {w200 ? 200 : 128, w200 ? 128 : 200};
+  Geometry first{};
+  for (int NW : widths) {
+    Geometry t = q;
+    t.N2 = NW;
+    t.stage2Bytes = 2u * (uint32_t)NW * 128u;
+    if (vBytes + 2u * t.stage2Bytes > ring) continue;
+    t.nS1 = nS1;
+    t.nS2 = (int)((ring - vBytes) / t.stage2Bytes); if (t.nS2 > kMaxS2) t.nS2 = kMaxS2;
+    t.ok = true;
+    if (!want_prefetch) return t;
+    if (!first.ok) first = t;
+    // both GEMMs give up stages (never below 2) until both prefetch warps have kMaxPf row slots
+    const uint32_t want = 2u * kMaxPf * row;
+    int s1 = t.nS1, s2 = t.nS2;
+    while (s1 > 2 && ring - (uint32_t)s1 * q.stage1Bytes < want) --s1;
+    while (s2 > 2 && ring - (vBytes + (uint32_t)s2 * t.stage2Bytes) < want) --s2;
+    uint32_t used = (uint32_t)s1 * q.stage1Bytes;
+    if (vBytes + (uint32_t)s2 * t.stage2Bytes > used) used = vBytes + (uint32_t)s2 * t.stage2Bytes;
+    int slots = (int)((ring - used) / (2u * row));
     if (slots > kMaxPf) slots = kMaxPf;
-    if (slots >= 2) { q.pf_slots = slots; q.nS1 = nS1; q.nS2 = nS2; q.pf_off = used; }
+    if (slots >= 2) { t.pf_slots = slots; t.nS1 = s1; t.nS2 = s2; t.pf_off = used; return t; }
   }
-  return q;
+  return first;
 }
 
 int launch_error() {
   const cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? KGE_OK : fail(KGE_ERR_CUDA, "k_fused launch: %s", cudaGetErrorString(e));
 }
-template <int NV>
+// k_fused<P>'s launch name carries the variant and the ring layout, so a profile says which one ran: GEMM1 width NV,
+// GEMM2 chunk NW, prefetch slots per warp and the number of V hand-off warps
+const char* pos_launch_name(int NV, int NW, int pf) {
+  static const int nvs[4] = {64, 128, 208, 256}, nws[2] = {128, 200};
+  static char names[4][2][kMaxPf + 1][96];
+  static std::once_flag once;
+  std::call_once(once, [] {
+    for (int a = 0; a < 4; ++a)
+      for (int b = 0; b < 2; ++b)
+        for (int f = 0; f <= kMaxPf; ++f)
+          snprintf(names[a][b][f], sizeof(names[a][b][f]), "k_fused<P: S=A.Bn^T, loss, GA=V.Bn> NV=%d NW=%d pf=%d hand=%d",
+                   nvs[a], nws[b], f, f > 0 ? 1 : 3);
+  });
+  const int a = NV == 64 ? 0 : NV == 128 ? 1 : NV == 208 ? 2 : 3;
+  return names[a][NW == 200][pf < 0 ? 0 : (pf > kMaxPf ? kMaxPf : pf)];
+}
+template <int NV, int NW>
 int launch_pos(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
-  if (int rc = smem_optin((const void*)k_fused_pos<NV>, smem)) return rc;
-  KGE_LAUNCH_NAMED(c, "k_fused<P: S=A.Bn^T, loss, GA=V.Bn>", (k_fused_pos<NV>), grid, kThreadsF, smem,
+  if (int rc = smem_optin((const void*)k_fused_pos<NV, NW>, smem)) return rc;
+  KGE_LAUNCH_NAMED(c, pos_launch_name(NV, NW, g.pf_slots), (k_fused_pos<NV, NW>), grid, kThreadsF, smem,
                    m[0], m[1], m[2], m[3], m[4], m[5], g);
   return launch_error();
+}
+template <int NV>
+int launch_pos(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
+  // geometry() never pairs N1 = 256 with NW = 200: the 128 KB V buffer and two 50 KB stages exceed the ring
+  if constexpr (NV < 256) {
+    if (g.N2 == 200) return launch_pos<NV, 200>(c, grid, smem, m, g);
+  }
+  return launch_pos<NV, 128>(c, grid, smem, m, g);
 }
 template <int NW, bool FLAT>
 int launch_neg_src(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
@@ -835,7 +925,7 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
   const bool P = mode == 0;
   const Geometry q = geometry(p, mode, pf != nullptr && ent != nullptr);
   if (!q.ok) return fail(KGE_ERR_UNSUPPORTED, "fused kernel: shape does not fit (N1=%d)", q.N1);
-  g.Rx = q.Rx; g.Ry = q.Ry; g.N1 = q.N1; g.nS1 = q.nS1; g.nS2 = q.nS2;
+  g.Rx = q.Rx; g.Ry = q.Ry; g.N1 = q.N1; g.N2 = q.N2; g.nS1 = q.nS1; g.nS2 = q.nS2;
   g.stage1Bytes = q.stage1Bytes; g.stage2Bytes = q.stage2Bytes;
   if (pf && ent && q.pf_slots >= 2) {
     static const int lag_env = getenv("KGE_B200_PF_LAG") ? atoi(getenv("KGE_B200_PF_LAG")) : 1;
@@ -847,7 +937,7 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
   }
   g.VhiT = w.VhiT; g.VloT = w.VloT; g.colpart = w.colpart; g.ncolpart = (p.Cs + kTileM - 1) / kTileM;
   g.dumpV = dumpV;
-  const size_t smem = kRingBytes + 1024;
+  const size_t smem = q.ringBytes + 1024;
   const int mtiles = (g.Rx + kTileM - 1) / kTileM;
   int grid = p.C * mtiles;
   if (grid > c.num_sms) grid = c.num_sms;
@@ -863,7 +953,7 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
     const long long rowsYT = (long long)p.C * slab_blocks(p.Ns) * p.D;
     if (tc_make_map(&m[0], w.Ahi, rowsX, 32, kTileM) || tc_make_map(&m[1], w.Alo, rowsX, 32, kTileM) ||
         tc_make_map(&m[2], w.Bhi, rowsY, 32, g.N1) || tc_make_map(&m[3], w.Blo, rowsY, 32, g.N1) ||
-        tc_make_map(&m[4], w.BhiT, rowsYT, 32, kWc) || tc_make_map(&m[5], w.BloT, rowsYT, 32, kWc))
+        tc_make_map(&m[4], w.BhiT, rowsYT, 32, g.N2) || tc_make_map(&m[5], w.BloT, rowsYT, 32, g.N2))
       return KGE_ERR_CUDA;
     return launch_width(c, true, grid, smem, m, g);
   }
