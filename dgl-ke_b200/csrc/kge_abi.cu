@@ -302,6 +302,7 @@ int carve(kge_context* h, const StepParams& p, StepWs* w, cudaStream_t stream, c
   const size_t B = (size_t)p.B, Nn = (size_t)p.Nn, U = (size_t)(p.U > 0 ? p.U : 0);
   const bool um = !opt.force_tiles && use_umma(h, p);
   const bool fused = p.fused != 0;
+  const FusedHilo hl = fused ? fused_hilo(p) : FusedHilo{false, false};
   // slab layout pads the blocked dimension to a multiple of 32 (+ one slab of slack for box overruns)
   const size_t sA = B * slab_blocks(p.D) * 32 + 8192, sB = Nn * slab_blocks(p.D) * 32 + 8192;
   const size_t sV = B * slab_blocks(p.Ns) * 32 + 8192;
@@ -319,10 +320,11 @@ int carve(kge_context* h, const StepParams& p, StepWs* w, cudaStream_t stream, c
       {&w->rowsum, B, true}, {&w->colsum, Nn, true}, {&w->pl, B, true}, {&w->nl, B, true}, {&w->wbar, 4, true},
       {&w->gsr, B, true}, {&w->gsn, Nn, true}, {&w->colpart, (size_t)ceil_div(p.Cs, 128) * Nn, fused},
       {&w->Mt, BD, p.model == KGE_RESCAL},
-      {&w->Ahi, sA, um}, {&w->Alo, sA, um}, {&w->Bhi, sB, um}, {&w->Blo, sB, um},
+      {&w->Ahi, sA, um && (!fused || hl.a)}, {&w->Alo, sA, um && (!fused || hl.a)}, {&w->Af, sA, fused && !hl.a},
+      {&w->Bhi, sB, um}, {&w->Blo, sB, um},
       {&w->Vhi, sV, um && !fused}, {&w->Vlo, sV, um && !fused},
       {&w->AhiT, sAT, um}, {&w->AloT, sAT, um}, {&w->BhiT, sBT, um}, {&w->BloT, sBT, um},
-      {&w->VhiT, sVT, um}, {&w->VloT, sVT, um},
+      {&w->VhiT, sVT, um && (!fused || hl.v)}, {&w->VloT, sVT, um && (!fused || hl.v)}, {&w->VT, sVT, fused},
       // U-dependent tail
       {&w->NC, U * p.D, p.use_nc != 0},
       {&w->regp, B + Nn + (U ? 2 * B : 0), true},

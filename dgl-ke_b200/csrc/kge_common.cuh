@@ -52,7 +52,7 @@ struct StepParams {
   int rel_deferred;  // 1: relation Adagrad is applied later from dense all-reduced buffers (multi-GPU)
   int rel_dense;     // 1: k_chain sums relation gradients per relation into ws.rg / ws.rgs (fused single-GPU step)
   int use_nc;        // 1: head/tail rows are read from the gathered copy NC (3-call API, sharded tables); 0: from the table
-  int fused;         // 1: contraction by the fused wgmma kernel (kge_fused.cu): operands exist only as TF32 hi/lo slabs
+  int fused;         // 1: contraction by the fused wgmma kernel (kge_fused.cu): operands exist only as slabs
   int hinge;         // 1: Hinge criterion (loss.py:10-17); 0: Logsigmoid == Logistic == BCE
   float margin;      // Hinge margin
   int pairwise;      // 1: criterion(pos_i - neg_ij, +1), plain mean over all (i, j) (loss.py:76-80)
@@ -104,7 +104,12 @@ struct StepWs {
   // contract over the rows of these matrices
   float *AhiT, *AloT; // [C][Cs/32][D][32]
   float *BhiT, *BloT; // [C][Ns/32][D][32]
-  float *VhiT, *VloT; // [C][Cs/32][Ns][32]   (fused step: written by mode P, the A operand of mode N)
+  float *VhiT, *VloT; // [C][Cs/32][Ns][32]   (stand-alone engine)
+  // fused step: the operands that are only ever the A operand of a fused GEMM, stored once as fp32 and split into TF32
+  // hi/lo in registers by the warp that issues the wgmma (kge_fused.cu); these replace Ahi/Alo and VhiT/VloT there,
+  // except next to a 256-wide accumulator (fused_hilo)
+  float* Af;          // [C][D/32][Cs][32]   (slab layout, written by k_prep, the A operand of GEMM1 in mode P)
+  float* VT;          // [C][Cs/32][Ns][32]   (written by mode P, the A operand of mode N)
 };
 
 struct BatchView {
@@ -231,8 +236,8 @@ inline size_t prep_stage_bytes(int D) { return (size_t)kPrepRows * prep_stage_st
 // the wgmma engine (transposed slabs) is offered only where k_prep's staging buffer fits one CTA: D <= 1796
 inline bool prep_stage_fits(int D) { return prep_stage_bytes(D) <= kSmemOptinMax; }
 
-// destination of an operand row: plain fp32 row-major and/or its TF32 hi/lo split in slab layout, and/or a copy in
-// shared memory (k_prep writes the transposed slabs from there)
+// destination of an operand row: plain fp32 row-major and/or its TF32 hi/lo split in slab layout and/or fp32 in slab
+// layout, and/or a copy in shared memory (k_prep writes the transposed slabs from there)
 struct RowOut {
   float* f32;        // row-major row pointer or null
   float* hi;         // slab-layout base pointers or null
@@ -240,15 +245,19 @@ struct RowOut {
   long long chunk;
   int nblk, R, row;
   float* stage;      // shared-memory row or null
+  float* slab;       // slab-layout base pointer of the unsplit fp32 row or null
 };
 __device__ __forceinline__ void row_store4(const RowOut& o, int col, float4 v) {
   if (o.f32) *reinterpret_cast<float4*>(o.f32 + col) = v;
-  if (o.hi) {
-    float4 h, l;
-    split_tf32_4(v, h, l);
+  if (o.hi || o.slab) {
     const long long off = slab_off(o.chunk, o.nblk, o.R, o.row, col);
-    *reinterpret_cast<float4*>(o.hi + off) = h;
-    *reinterpret_cast<float4*>(o.lo + off) = l;
+    if (o.slab) *reinterpret_cast<float4*>(o.slab + off) = v;
+    if (o.hi) {
+      float4 h, l;
+      split_tf32_4(v, h, l);
+      *reinterpret_cast<float4*>(o.hi + off) = h;
+      *reinterpret_cast<float4*>(o.lo + off) = l;
+    }
   }
   if (o.stage) *reinterpret_cast<float4*>(o.stage + col) = v;
 }
@@ -442,6 +451,10 @@ struct FusedPrefetch {
 bool fused_supported(const StepParams&);
 // row slots per prefetch warp the shape leaves room for (< 2: none)
 int fused_prefetch_slots(const StepParams& p, int mode);
+// A operands of the fused kernels that travel as TF32 hi/lo slabs instead of fp32 (their 256-wide variants): the
+// a-side (Ahi/Alo instead of Af) and the coefficients (VhiT/VloT as well as VT: without prefetch slots only)
+struct FusedHilo { bool a, v; };
+FusedHilo fused_hilo(const StepParams& p);
 int fused_launch(const LaunchCtx&, const StepParams&, const StepWs&, int mode, const float* wt, float* dumpS, float* dumpV,
                  const TableView* ent, const long long* neg_ids, const FusedPrefetch* pf);
 

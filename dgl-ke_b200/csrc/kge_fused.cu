@@ -6,26 +6,30 @@
 //               (tensor cores, V loaded per k-step as the REGISTER A operand, split into TF32 hi/lo) -> epilogue.
 //               Replaces create_neg (score_fun.py:91-108,268-286,345-376,427-449), LossGenerator.get_total_loss
 //               (loss.py:69-98) and the dL/da half of loss.backward().  The score matrix S never leaves the SM; V leaves
-//               it once, as the transposed TF32 hi/lo slabs V^T[c][i / 32][j][i % 32] plus per-tile column sums
-//               sum_i V_ij, for k_fused<N>; spare warps write both from the shared-memory copy while GEMM2 runs.
+//               it once, as the transposed fp32 slab V^T[c][i / 32][j][i % 32] plus per-tile column sums sum_i V_ij,
+//               for k_fused<N>; spare warps write both from the shared-memory copy while GEMM2 runs.
 //   k_fused<N>  rows = negatives j:  G_neg = V^T.A - colsum*b + reg'(b), mean(G_neg^2)  (the dL/db half of
 //               loss.backward() plus phase 1 of ExternalEmbedding.update for the negatives, tensor_models.py:316-328).
-//               One pipelined GEMM over K = Cs with both operands from shared memory: V^T slabs (written by k_fused<P>)
-//               and the transposed A slabs (written by k_prep).
+//               One pipelined GEMM over K = Cs: the V^T slab (written by k_fused<P>) as the register A operand and the
+//               transposed A slabs (written by k_prep) from shared memory.
 //
-// Handing V over costs 2 x 4 B x C x Cs x Ns of HBM traffic each way (23.6 MB at 66 chunks of 200 x 200); recomputing
-// it in the second orientation cost a whole K = D GEMM per chunk plus the loss epilogue, and an S accumulator that
+// Handing V over costs 4 B x C x Cs x Ns of HBM traffic each way (11.8 MB at 66 chunks of 200 x 200); recomputing it
+// in the second orientation cost a whole K = D GEMM per chunk plus the loss epilogue, and an S accumulator that
 // crowded the register file.  fp32 fidelity: operands are TF32 hi/lo pairs and every k-step issues hi*hi + hi*lo +
-// lo*hi (3xTF32, fp32 accumulation).  wgmma reads TF32 operands K-major only: GEMMs that contract over the rows of a
-// matrix take its transposed slabs (kge_common.cuh:slabT_off).
+// lo*hi (3xTF32, fp32 accumulation).  B operands come from shared memory as hi/lo slabs.  An A operand is loaded as
+// fp32 and split by the issuing thread into the register fragment (a_frag), so it crosses HBM once instead of twice --
+// except next to a 256-column accumulator, where two fragment sets do not fit the register file (ptxas serialises or
+// spills): those variants (kRegA false) read A as hi/lo slabs from shared memory, as the B operand.  wgmma reads TF32 operands from shared memory K-major only: GEMMs that contract over the rows of a matrix
+// take its transposed slabs (kge_common.cuh:slabT_off).
 //
 // CTA = 384 threads: warpgroups 0 and 1 (warps 0-7) each own 64 rows of the 128-row tile -- MMA issue and epilogue on
 // the accumulator fragment, a row lives in the 4 lanes of a quad; warp 8 TMA producer, warps 10-11 prefetch the next
 // step's rows; in k_fused<P> warp 9 (and 10-11 when they do not prefetch) write the V hand-off.  Persistent over
 // (chunk, 128-row tile) work items.
-// Shared memory: one ring.  k_fused<P> (223 KB, 192 KB with prefetch slots) uses it as nS1 stages {X_hi,X_lo,Y_hi,Y_lo} for GEMM1, then as
+// Shared memory: one ring.  k_fused<P> (223 KB, 192 KB with prefetch slots) uses it as nS1 stages {X,Y_hi,Y_lo} for GEMM1, then as
 // the V buffer followed by nS2 stages {Y^T_hi,Y^T_lo} for GEMM2, whose output is produced in chunks of NW columns;
-// k_fused<N> (192 KB) as nS stages {V^T_hi,V^T_lo,A^T_hi,A^T_lo} of one output-column chunk of width NW.
+// k_fused<N> (192 KB) as nS stages {V^T,A^T_hi,A^T_lo} of one output-column chunk of width NW.  X and V^T are fp32, or
+// hi/lo pairs {X_hi,X_lo} / {V^T_hi,V^T_lo} in the 256-wide variants.
 #include <cuda.h>
 #include <cstdio>
 #include <cstdlib>
@@ -63,7 +67,8 @@ struct FusedArgs {
   int nblkD;             // 32-column slab blocks of D
   int nS1, nS2;          // P: GEMM1 / GEMM2 stages;  N: nS1 stages
   uint32_t stage1Bytes, stage2Bytes;
-  float *VhiT, *VloT;    // [C][Cs/32][Ns][32] coefficients V_ij as TF32 hi/lo (P writes, N reads)
+  float* VT;             // [C][Cs/32][Ns][32] coefficients V_ij, fp32 (P writes, N reads) ...
+  float *VhiT, *VloT;    //   ... or as TF32 hi/lo when k_fused<N> runs 256 columns wide (VhiT set: P writes these)
   float* colpart;        // [ceil(Cs/128)][C*Ns] per-tile column sums sum_i V_ij (TransE_l2; P writes, N reads)
   int ncolpart;          // N: number of those partials
   // mode P
@@ -165,6 +170,9 @@ __device__ __forceinline__ void prefetch_rows(const FusedArgs& g, uint8_t* ring,
   __syncwarp();
 }
 
+// A 256-wide accumulator leaves no room for register fragments: such variants use k_reg_a() false
+__host__ __device__ constexpr bool k_reg_a(int n) { return n < 256; }
+
 // one k-block of a GEMM with both operands in shared memory: KS k-steps of 8, each hi*hi + hi*lo + lo*hi, as one wgmma
 // group.  A guard between the fence and the commit would make ptxas insert warpgroup arrives of its own, so callers
 // switch over the k-step count.
@@ -179,6 +187,62 @@ __device__ __forceinline__ void kblock_3xtf32(float (&acc)[NW / 2], uint64_t dXh
     wgmma_ss<NW>(acc, dXl + o, dYh + o, 1u);
   }
   wgmma_commit();
+}
+
+__device__ __forceinline__ float lds_f32(uint32_t a) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory");
+  return v;
+}
+
+// The register A fragment of k-step ks from an fp32 stage of 128 rows x 32 floats (K-major, TMA 128-byte swizzle: the
+// 16-byte chunk c of row r sits at chunk position c ^ (r & 7)), split into TF32 hi/lo.  Thread (g = lane / 4,
+// q = lane % 4) of MMA warp w reads (r, k = 8 ks + q), (r + 8, q), (r, q + 4), (r + 8, q + 4) for r = 16 w + g, i.e.
+// float q of chunk 2 ks (+1 for q + 4).  r and r + 8 share r & 7 = g, so each of the four loads reaches bank
+// 4 ((2 ks [+1]) ^ g) + q: the 8 values of g give 8 distinct chunk positions and q the 4 words in each, so the 32 lanes
+// hit 32 distinct banks.  `row` is the shared address of row r.
+__device__ __forceinline__ void a_frag(uint32_t row, int ks, int g, int q, uint32_t (&ah)[4], uint32_t (&al)[4]) {
+  const uint32_t c0 = row + (uint32_t)(((((2 * ks) ^ g) << 2) + q) << 2);
+  const uint32_t c1 = row + (uint32_t)(((((2 * ks + 1) ^ g) << 2) + q) << 2);
+  const float a[4] = {lds_f32(c0), lds_f32(c0 + 1024u), lds_f32(c1), lds_f32(c1 + 1024u)};
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    float hi, lo;
+    split_tf32(a[r], hi, lo);
+    ah[r] = __float_as_uint(hi); al[r] = __float_as_uint(lo);
+  }
+}
+
+// one k-step hi*hi + hi*lo + lo*hi as one wgmma group, the A fragment in registers
+template <int N>
+__device__ __forceinline__ void kstep_rs(float (&acc)[N / 2], const uint32_t (&ah)[4], const uint32_t (&al)[4],
+                                         uint64_t dYh, uint64_t dYl) {
+  wgmma_fence();
+  wgmma_rs<N>(acc, ah, dYh, 1u);
+  wgmma_rs<N>(acc, ah, dYl, 1u);
+  wgmma_rs<N>(acc, al, dYh, 1u);
+  wgmma_commit();
+}
+
+// One k-block of KS k-steps of 8 whose A operand is an fp32 stage (a_frag) and whose B operand is a hi/lo pair of
+// shared-memory slabs: one wgmma group per k-step, at most two in flight.  Two fragment sets alternate and a set is
+// re-written only once the group that reads it has retired; every k-block but the last has 4 k-steps, so k-step ks
+// always takes set ks & 1.  `release`: the previous k-block's stage, handed back once the first group of this one is
+// issued and the previous one's last group has retired (its ld.shared reads are done before its wgmmas are issued).
+// A guard between a fence and a commit would make ptxas insert warpgroup arrives of its own, so callers switch over the
+// k-step count.
+template <int N, int KS>
+__device__ __forceinline__ void kblock_rs(float (&acc)[N / 2], uint32_t (&ah)[2][4], uint32_t (&al)[2][4], uint32_t row,
+                                          int g, int q, uint64_t dYh, uint64_t dYl, uint64_t* release, int lane) {
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    a_frag(row, ks, g, q, ah[ks & 1], al[ks & 1]);
+    const uint64_t o = (uint64_t)(ks * 2);     // K-major: +32 bytes per k-step inside the 128-byte swizzle span
+    kstep_rs<N>(acc, ah[ks & 1], al[ks & 1], dYh + o, dYl + o);
+    wgmma_wait<1>();                           // the previous k-step has retired: its fragment set is free
+    reg_fence(ah[(ks + 1) & 1]); reg_fence(al[(ks + 1) & 1]);
+    if (ks == 0 && release && lane == 0) mbar_arrive(release);
+  }
 }
 
 // ================================ k_fused<P> ================================
@@ -208,11 +272,7 @@ __device__ __forceinline__ void pos_kstep(float (&acc2)[NW / 2], uint32_t (&ah)[
     split_tf32(a[r], hi, lo);
     ah[r] = __float_as_uint(hi); al[r] = __float_as_uint(lo);
   }
-  wgmma_fence();
-  wgmma_rs<NW>(acc2, ah, dYh, 1u);
-  wgmma_rs<NW>(acc2, ah, dYl, 1u);
-  wgmma_rs<NW>(acc2, al, dYh, 1u);
-  wgmma_commit();
+  kstep_rs<NW>(acc2, ah, al, dYh, dYl);
 }
 
 // this thread's first row inside the 128-row tile (16 per warp, lane / 4; the second is 8 further): read from %tid.x
@@ -226,7 +286,7 @@ __device__ __forceinline__ int tile_row() {
 
 template <int NV, int NW>
 __global__ void __launch_bounds__(kThreadsF, 1)
-k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUtensorMap mXl,
+k_fused_pos(const __grid_constant__ CUtensorMap mX, const __grid_constant__ CUtensorMap mXl,   // mXl: !k_reg_a(NV) only
             const __grid_constant__ CUtensorMap mYh1, const __grid_constant__ CUtensorMap mYl1,
             const __grid_constant__ CUtensorMap mYh2, const __grid_constant__ CUtensorMap mYl2, FusedArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -248,6 +308,7 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
   const int nkb2 = (g.Ry + 31) >> 5;
   const int nchunks = (g.D + NW - 1) / NW;
   constexpr uint32_t yBytes1 = (uint32_t)NV * 128u;
+  constexpr uint32_t xBytes1 = k_reg_a(NV) ? 16384u : 32768u;      // X as fp32, or as hi + lo
   constexpr uint32_t yBytes2 = (uint32_t)NW * 128u;
   const bool l2 = g.model == KGE_TRANSE_L2;
   // the hand-off warps: warp 9, and warps 10-11 when they do not prefetch; they meet the MMA warps at named barrier 2
@@ -262,8 +323,8 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (warp == kProducerWarp && lane == 0) {
-    tma_prefetch_desc(&mXh); tma_prefetch_desc(&mXl); tma_prefetch_desc(&mYh1);
-    tma_prefetch_desc(&mYl1); tma_prefetch_desc(&mYh2); tma_prefetch_desc(&mYl2);
+    tma_prefetch_desc(&mX); if (!k_reg_a(NV)) tma_prefetch_desc(&mXl); tma_prefetch_desc(&mYh1); tma_prefetch_desc(&mYl1);
+    tma_prefetch_desc(&mYh2); tma_prefetch_desc(&mYl2);
   }
   __syncthreads();
 
@@ -288,11 +349,11 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
         const int yx = (c * g.nblkD + kb) * g.Rx + m0;
         const int yy = (c * g.nblkD + kb) * g.Ry;
         if (elect_one()) {
-          mbar_expect_tx(&full1[s], 2u * 16384u + 2u * yBytes1);
-          tma_load_2d(st, &mXh, &full1[s], 0, yx);
-          tma_load_2d(st + 16384, &mXl, &full1[s], 0, yx);
-          tma_load_2d(st + 32768, &mYh1, &full1[s], 0, yy);
-          tma_load_2d(st + 32768 + yBytes1, &mYl1, &full1[s], 0, yy);
+          mbar_expect_tx(&full1[s], xBytes1 + 2u * yBytes1);
+          tma_load_2d(st, &mX, &full1[s], 0, yx);
+          if (!k_reg_a(NV)) tma_load_2d(st + 16384, &mXl, &full1[s], 0, yx);
+          tma_load_2d(st + xBytes1, &mYh1, &full1[s], 0, yy);
+          tma_load_2d(st + xBytes1 + yBytes1, &mYl1, &full1[s], 0, yy);
         }
         __syncwarp();
       }
@@ -316,9 +377,9 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
     }
   } else if (warp - kHandoffWarp < nhand) {
     // ================================ V hand-off to k_fused<N> ================================
-    // V_ij = coef_ij / den_i as TF32 hi/lo in the transposed slabs V^T[c][i / 32][j][i % 32]: per column j and 32-row
-    // block, one lane per row, so every store is a whole 128-byte line; rows i >= Cs are not written (k_fused<N> never
-    // reads them).  TransE_l2 also needs sum_i V_ij over the tile: each lane adds its rows of the blocks in order, then
+    // V_ij = coef_ij / den_i in the transposed fp32 slab V^T[c][i / 32][j][i % 32] (or its hi/lo pair, for a 256-wide
+    // k_fused<N>): per column j and 32-row block, one lane per row, so every store is a whole 128-byte line; rows i >= Cs are not written (k_fused<N> never reads
+    // them).  TransE_l2 also needs sum_i V_ij over the tile: each lane adds its rows of the blocks in order, then
     // a fixed butterfly over the lanes.  Both are read from the shared-memory copy while the MMA warps run GEMM2.
     const int hw = warp - kHandoffWarp;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -339,10 +400,14 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
         for (int b = 0; b < kTileM / 32; ++b) {
           const int i = 32 * b + lane;
           if (i < rows) {
-            float hi, lo;
-            split_tf32(v[b], hi, lo);
             const long long o = slabT_off(c, g.Rx, g.Ry, m0 + i, j);
-            g.VhiT[o] = hi; g.VloT[o] = lo;
+            if (g.VhiT) {
+              float hi, lo;
+              split_tf32(v[b], hi, lo);
+              g.VhiT[o] = hi; g.VloT[o] = lo;
+            } else {
+              g.VT[o] = v[b];
+            }
           }
           s += v[b];
         }
@@ -362,7 +427,7 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
   } else {
     // ================================ MMA + epilogue warps 0..7 ================================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int wg = warp >> 2, q = lane & 3;
+    const int q = lane & 3;
     const int et = threadIdx.x;                   // 0..255
     uint32_t n1 = 0, n2 = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -376,30 +441,53 @@ k_fused_pos(const __grid_constant__ CUtensorMap mXh, const __grid_constant__ CUt
       float rscal[2];                             // 1 / softmax denominator (or 1 / Ns) of the two rows
       {
       float acc[NV / 2];                          // S -> V: rows rloc (+8), columns 8 j + 2 q + {0, 1}
-      // ---- GEMM1: S = X . Y^T, K = D ----
+      // ---- GEMM1: S = X . Y^T, K = D; X (fp32) as the register A operand ----
 #pragma unroll
       for (int i = 0; i < NV / 2; ++i) acc[i] = 0.f;
-      for (int kb = 0; kb < nkb1; ++kb, ++n1) {
-        const uint32_t s = n1 % g.nS1;
-        mbar_wait(&full1[s], (n1 / g.nS1) & 1);
-        const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
-        const uint64_t dXh = make_desc(st + wg * 8192u), dXl = make_desc(st + 16384u + wg * 8192u);
-        const uint64_t dYh = make_desc(st + 32768u), dYl = make_desc(st + 32768u + yBytes1);
-        const int kleft = g.D - kb * 32;
-        const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
-        // one straight-line fence .. wgmma .. commit sequence per k-step count (see neg_kblock)
-        switch (ksteps) {
-          case 4: kblock_3xtf32<NV, 4>(acc, dXh, dXl, dYh, dYl); break;
-          case 3: kblock_3xtf32<NV, 3>(acc, dXh, dXl, dYh, dYl); break;
-          case 2: kblock_3xtf32<NV, 2>(acc, dXh, dXl, dYh, dYl); break;
-          default: kblock_3xtf32<NV, 1>(acc, dXh, dXl, dYh, dYl); break;
+      if constexpr (k_reg_a(NV)) {
+        uint32_t ah[2][4], al[2][4];
+        const int g8 = (lane >> 2);
+        for (int kb = 0; kb < nkb1; ++kb, ++n1) {
+          const uint32_t s = n1 % g.nS1;
+          mbar_wait(&full1[s], (n1 / g.nS1) & 1);
+          const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
+          const uint32_t xrow = st + (uint32_t)(16 * warp + g8) * 128u;
+          const uint64_t dYh = make_desc(st + xBytes1), dYl = make_desc(st + xBytes1 + yBytes1);
+          const int kleft = g.D - kb * 32;
+          const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
+          uint64_t* rel = kb > 0 ? &empty1[(n1 - 1) % g.nS1] : nullptr;
+          switch (ksteps) {
+            case 4: kblock_rs<NV, 4>(acc, ah, al, xrow, g8, q, dYh, dYl, rel, lane); break;
+            case 3: kblock_rs<NV, 3>(acc, ah, al, xrow, g8, q, dYh, dYl, rel, lane); break;
+            case 2: kblock_rs<NV, 2>(acc, ah, al, xrow, g8, q, dYh, dYl, rel, lane); break;
+            default: kblock_rs<NV, 1>(acc, ah, al, xrow, g8, q, dYh, dYl, rel, lane); break;
+          }
         }
-        if (kb > 0) {
-          wgmma_wait<1>();                           // the previous k-block has retired: its stage is free
-          if (lane == 0) mbar_arrive(&empty1[(n1 - 1) % g.nS1]);
+        wgmma_wait<0>();
+        reg_fence(ah[0]); reg_fence(ah[1]); reg_fence(al[0]); reg_fence(al[1]);
+      } else {
+        const int wg = warp >> 2;
+        for (int kb = 0; kb < nkb1; ++kb, ++n1) {
+          const uint32_t s = n1 % g.nS1;
+          mbar_wait(&full1[s], (n1 / g.nS1) & 1);
+          const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
+          const uint64_t dXh = make_desc(st + wg * 8192u), dXl = make_desc(st + 16384u + wg * 8192u);
+          const uint64_t dYh = make_desc(st + xBytes1), dYl = make_desc(st + xBytes1 + yBytes1);
+          const int kleft = g.D - kb * 32;
+          const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
+          switch (ksteps) {
+            case 4: kblock_3xtf32<NV, 4>(acc, dXh, dXl, dYh, dYl); break;
+            case 3: kblock_3xtf32<NV, 3>(acc, dXh, dXl, dYh, dYl); break;
+            case 2: kblock_3xtf32<NV, 2>(acc, dXh, dXl, dYh, dYl); break;
+            default: kblock_3xtf32<NV, 1>(acc, dXh, dXl, dYh, dYl); break;
+          }
+          if (kb > 0) {
+            wgmma_wait<1>();                           // the previous k-block has retired: its stage is free
+            if (lane == 0) mbar_arrive(&empty1[(n1 - 1) % g.nS1]);
+          }
         }
+        wgmma_wait<0>();
       }
-      wgmma_wait<0>();
       if (lane == 0) mbar_arrive(&empty1[(n1 - 1) % g.nS1]);
       reg_fence(acc);
       epi_bar();                                  // both warpgroups' GEMM1 has retired: the V buffer may overwrite the stages
@@ -569,7 +657,7 @@ constexpr int kNegEpiLoads = 16;
 // otherwise as hi + lo from the slabs.  The source is fixed per launch, so the column loop never branches on it.
 template <int NW, bool FLAT>
 __global__ void __launch_bounds__(kThreadsF, 1)
-k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUtensorMap mVl,
+k_fused_neg(const __grid_constant__ CUtensorMap mV, const __grid_constant__ CUtensorMap mVl,   // mVl: !k_reg_a(NW) only
             const __grid_constant__ CUtensorMap mAh, const __grid_constant__ CUtensorMap mAl, FusedArgs g) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full[kMaxS1], empty[kMaxS1];
@@ -584,6 +672,7 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
   const int nch = (g.D + NW - 1) / NW;
   constexpr uint32_t aBytes = (uint32_t)kTileM * 128u;
   constexpr uint32_t bBytes = (uint32_t)NW * 128u;
+  constexpr uint32_t vBytes = k_reg_a(NW) ? aBytes : 2u * aBytes;     // V^T as fp32, or as hi + lo
   const bool l2 = g.model == KGE_TRANSE_L2;
 
   if (threadIdx.x == 0) {
@@ -592,7 +681,7 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (warp == kProducerWarp && lane == 0) {
-    tma_prefetch_desc(&mVh); tma_prefetch_desc(&mVl); tma_prefetch_desc(&mAh); tma_prefetch_desc(&mAl);
+    tma_prefetch_desc(&mV); if (!k_reg_a(NW)) tma_prefetch_desc(&mVl); tma_prefetch_desc(&mAh); tma_prefetch_desc(&mAl);
   }
   __syncthreads();
 
@@ -612,11 +701,11 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
           const int yv = (c * nkb + kb) * g.Rx + m0;
           const int ya = (c * nkb + kb) * g.D + ch * NW;
           if (elect_one()) {
-            mbar_expect_tx(&full[s], 2u * aBytes + 2u * bBytes);
-            tma_load_2d(st, &mVh, &full[s], 0, yv);
-            tma_load_2d(st + aBytes, &mVl, &full[s], 0, yv);
-            tma_load_2d(st + 2 * aBytes, &mAh, &full[s], 0, ya);
-            tma_load_2d(st + 2 * aBytes + bBytes, &mAl, &full[s], 0, ya);
+            mbar_expect_tx(&full[s], vBytes + 2u * bBytes);
+            tma_load_2d(st, &mV, &full[s], 0, yv);
+            if (!k_reg_a(NW)) tma_load_2d(st + aBytes, &mVl, &full[s], 0, yv);
+            tma_load_2d(st + vBytes, &mAh, &full[s], 0, ya);
+            tma_load_2d(st + vBytes + bBytes, &mAl, &full[s], 0, ya);
           }
           __syncwarp();
         }
@@ -635,12 +724,15 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const int c = tile / mtiles, m0 = (tile % mtiles) * kTileM;
       if (g.dumpV) {
-        // test hook: the coefficients this tile reads, [C*Ns, Cs] (hi + lo)
+        // test hook: the coefficients this tile reads, [C*Ns, Cs], as the MMAs see them (hi + lo of the split)
         for (int e = et; e < kTileM * g.Ry; e += 256) {
           const int j = m0 + e / g.Ry, i = e % g.Ry;
           if (j >= g.Rx) break;
           const long long o = slabT_off(c, g.Ry, g.Rx, i, j);
-          g.dumpV[((long long)c * g.Rx + j) * g.Ry + i] = g.VhiT[o] + g.VloT[o];
+          float hi, lo;
+          if (k_reg_a(NW)) split_tf32(g.VT[o], hi, lo);
+          else { hi = g.VhiT[o]; lo = g.VloT[o]; }
+          g.dumpV[((long long)c * g.Rx + j) * g.Ry + i] = hi + lo;
         }
       }
       // sum_i V_ij of this thread's two rows: the per-tile partials of k_fused<P>, added in a fixed order
@@ -698,30 +790,51 @@ k_fused_neg(const __grid_constant__ CUtensorMap mVh, const __grid_constant__ CUt
         float acc[NW / 2];                        // rows rloc (+8), columns d0 + 8 j + 2 q + {0, 1}
 #pragma unroll
         for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
-        for (int kb = 0; kb < nkb; ++kb, ++n) {
-          const uint32_t s = n % g.nS1;
-          mbar_wait(&full[s], (n / g.nS1) & 1);
-          const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
-          const uint64_t dVh = make_desc(st + wg * 8192u), dVl = make_desc(st + aBytes + wg * 8192u);
-          const uint64_t dAh = make_desc(st + 2 * aBytes), dAl = make_desc(st + 2 * aBytes + bBytes);
-          // K = Cs is a multiple of 8: the partial last block runs its whole k-steps and never reads the padding
-          const int kleft = g.Ry - kb * 32;
-          const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
-          // one straight-line fence .. wgmma .. commit sequence per k-step count: a guard between the fence and the
-          // commit makes ptxas insert warpgroup arrives of its own
-          switch (ksteps) {
-            case 4: kblock_3xtf32<NW, 4>(acc, dVh, dVl, dAh, dAl); break;
-            case 3: kblock_3xtf32<NW, 3>(acc, dVh, dVl, dAh, dAl); break;
-            case 2: kblock_3xtf32<NW, 2>(acc, dVh, dVl, dAh, dAl); break;
-            default: kblock_3xtf32<NW, 1>(acc, dVh, dVl, dAh, dAl); break;
+        if constexpr (k_reg_a(NW)) {
+          uint32_t ah[2][4], al[2][4];
+          for (int kb = 0; kb < nkb; ++kb, ++n) {
+            const uint32_t s = n % g.nS1;
+            mbar_wait(&full[s], (n / g.nS1) & 1);
+            const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
+            const uint32_t vrow = st + (uint32_t)(16 * warp + (lane >> 2)) * 128u;
+            const uint64_t dAh = make_desc(st + vBytes), dAl = make_desc(st + vBytes + bBytes);
+            // K = Cs is a multiple of 8: the partial last block runs its whole k-steps and never reads the padding
+            const int kleft = g.Ry - kb * 32;
+            const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
+            uint64_t* rel = kb > 0 ? &empty[(n - 1) % g.nS1] : nullptr;
+            switch (ksteps) {
+              case 4: kblock_rs<NW, 4>(acc, ah, al, vrow, lane >> 2, q, dAh, dAl, rel, lane); break;
+              case 3: kblock_rs<NW, 3>(acc, ah, al, vrow, lane >> 2, q, dAh, dAl, rel, lane); break;
+              case 2: kblock_rs<NW, 2>(acc, ah, al, vrow, lane >> 2, q, dAh, dAl, rel, lane); break;
+              default: kblock_rs<NW, 1>(acc, ah, al, vrow, lane >> 2, q, dAh, dAl, rel, lane); break;
+            }
           }
-          if (kb > 0) {
-            wgmma_wait<1>();                           // the previous k-block has retired: its stage is free
-            if (lane == 0) mbar_arrive(&empty[(n - 1) % g.nS1]);
+          if (early) load_b(0, d0, 0);
+          wgmma_wait<0>();
+          reg_fence(ah[0]); reg_fence(ah[1]); reg_fence(al[0]); reg_fence(al[1]);
+        } else {
+          for (int kb = 0; kb < nkb; ++kb, ++n) {
+            const uint32_t s = n % g.nS1;
+            mbar_wait(&full[s], (n / g.nS1) & 1);
+            const uint32_t st = smem_u32(ring + (size_t)s * g.stage1Bytes);
+            const uint64_t dVh = make_desc(st + wg * 8192u), dVl = make_desc(st + aBytes + wg * 8192u);
+            const uint64_t dAh = make_desc(st + vBytes), dAl = make_desc(st + vBytes + bBytes);
+            const int kleft = g.Ry - kb * 32;
+            const int ksteps = kleft >= 32 ? 4 : (kleft >> 3);
+            switch (ksteps) {
+              case 4: kblock_3xtf32<NW, 4>(acc, dVh, dVl, dAh, dAl); break;
+              case 3: kblock_3xtf32<NW, 3>(acc, dVh, dVl, dAh, dAl); break;
+              case 2: kblock_3xtf32<NW, 2>(acc, dVh, dVl, dAh, dAl); break;
+              default: kblock_3xtf32<NW, 1>(acc, dVh, dVl, dAh, dAl); break;
+            }
+            if (kb > 0) {
+              wgmma_wait<1>();                         // the previous k-block has retired: its stage is free
+              if (lane == 0) mbar_arrive(&empty[(n - 1) % g.nS1]);
+            }
           }
+          if (early) load_b(0, d0, 0);
+          wgmma_wait<0>();
         }
-        if (early) load_b(0, d0, 0);
-        wgmma_wait<0>();
         if (lane == 0) mbar_arrive(&empty[(n - 1) % g.nS1]);
         reg_fence(acc);
         // chunk epilogue from the fragment (the producer is already filling the next chunk's stages)
@@ -772,7 +885,11 @@ bool fused_supported(const StepParams& p) {
 
 // mode 0 (P): S = A.Bn^T -> loss, coefficients V -> GA, V^T slabs;  mode 1 (N): G_neg = V^T.A (+ mean square)
 namespace {
-// GEMM stage geometry of one mode + what the ring leaves for prefetch row slots
+// GEMM stage geometry of one mode + what the ring leaves for prefetch row slots.  A GEMM1 / k_fused<N> stage holds its
+// A operand (kTileM x 128 B) once, as fp32, or as hi + lo in the 256-wide variants; layouts with prefetch slots are
+// sized as if it always took a hi and a lo copy, so that their stage and slot counts do not depend on that.
+constexpr uint32_t kLoBytes = (uint32_t)kTileM * 128u;
+uint32_t stage1_bytes(int n) { return (k_reg_a(n) ? 1u : 2u) * kLoBytes + 2u * (uint32_t)n * 128u; }
 struct Geometry { int Rx, Ry, N1, N2, nS1, nS2, pf_slots; uint32_t ringBytes, stage1Bytes, stage2Bytes, pf_off; bool ok; };
 
 // k_fused<N>: the output-column chunk NW.  A pass over K streams the tile's V^T (128 rows) and the chunk's A^T (NW rows),
@@ -799,17 +916,18 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
     q.Rx = p.Ns; q.Ry = p.Cs;
     q.ringBytes = kRingBytes;
     q.N1 = neg_chunk_width(p.D, want_prefetch);
-    q.stage1Bytes = 2u * kTileM * 128u + 2u * (uint32_t)q.N1 * 128u;
+    q.stage1Bytes = stage1_bytes(q.N1);
     q.nS1 = (int)(kRingBytes / q.stage1Bytes); if (q.nS1 > kMaxS1) q.nS1 = kMaxS1;
     q.ok = q.nS1 >= 2;
     if (q.ok && want_prefetch) {
       // the GEMM gives up stages (never below 2) until both prefetch warps have kMaxPf row slots
-      int nS = q.nS1;
-      while (nS > 2 && kRingBytes - (uint32_t)nS * q.stage1Bytes < 2u * kMaxPf * row) --nS;
-      const uint32_t used = (uint32_t)nS * q.stage1Bytes;
+      const uint32_t fp = stage1_bytes(q.N1) + (k_reg_a(q.N1) ? kLoBytes : 0u);
+      int nS = (int)(kRingBytes / fp); if (nS > kMaxS1) nS = kMaxS1;
+      while (nS > 2 && kRingBytes - (uint32_t)nS * fp < 2u * kMaxPf * row) --nS;
+      const uint32_t used = (uint32_t)nS * fp;
       int slots = (int)((kRingBytes - used) / (2u * row));
       if (slots > kMaxPf) slots = kMaxPf;
-      if (slots >= 2) { q.pf_slots = slots; q.nS1 = nS; q.pf_off = used; }
+      if (slots >= 2 && nS >= 2) { q.pf_slots = slots; q.nS1 = nS; q.pf_off = used; }
     }
     return q;
   }
@@ -821,8 +939,9 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
   // may opt in to.
   const uint32_t ring = want_prefetch ? kRingBytes : kRingBytesP;
   q.ringBytes = ring;
-  q.stage1Bytes = 2u * 16384u + 2u * (uint32_t)q.N1 * 128u;
-  int nS1 = (int)(ring / q.stage1Bytes); if (nS1 > kMaxS1) nS1 = kMaxS1;
+  q.stage1Bytes = stage1_bytes(q.N1);
+  const uint32_t fp1 = (want_prefetch && k_reg_a(q.N1)) ? q.stage1Bytes + kLoBytes : q.stage1Bytes;
+  int nS1 = (int)(ring / fp1); if (nS1 > kMaxS1) nS1 = kMaxS1;
   if (nS1 < 2) return q;
   // GEMM2 needs the V buffer (N1 / 8 k-steps x 512 B per MMA warp) ahead of its stages.  Its output-column chunk NW:
   // a chunk streams NW rows of Bn^T per k-block and issues NW columns of MMAs, so ceil(D / NW) * NW should be least
@@ -846,9 +965,9 @@ Geometry geometry(const StepParams& p, int mode, bool want_prefetch) {
     // both GEMMs give up stages (never below 2) until both prefetch warps have kMaxPf row slots
     const uint32_t want = 2u * kMaxPf * row;
     int s1 = t.nS1, s2 = t.nS2;
-    while (s1 > 2 && ring - (uint32_t)s1 * q.stage1Bytes < want) --s1;
+    while (s1 > 2 && ring - (uint32_t)s1 * fp1 < want) --s1;
     while (s2 > 2 && ring - (vBytes + (uint32_t)s2 * t.stage2Bytes) < want) --s2;
-    uint32_t used = (uint32_t)s1 * q.stage1Bytes;
+    uint32_t used = (uint32_t)s1 * fp1;
     if (vBytes + (uint32_t)s2 * t.stage2Bytes > used) used = vBytes + (uint32_t)s2 * t.stage2Bytes;
     int slots = (int)((ring - used) / (2u * row));
     if (slots > kMaxPf) slots = kMaxPf;
@@ -895,7 +1014,11 @@ int launch_pos(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, 
 template <int NW, bool FLAT>
 int launch_neg_src(const LaunchCtx& c, int grid, size_t smem, const CUtensorMap* m, const FusedArgs& g) {
   if (int rc = smem_optin((const void*)k_fused_neg<NW, FLAT>, smem)) return rc;
-  KGE_LAUNCH_NAMED(c, "k_fused<N: G_neg=V^T.A, mean sq>", (k_fused_neg<NW, FLAT>), grid, kThreadsF, smem, m[0], m[1], m[2], m[3], g);
+  // the launch name carries the output-column chunk width, so a profile says which variant ran
+  static char name[64];
+  static std::once_flag once;
+  std::call_once(once, [] { snprintf(name, sizeof(name), "k_fused<N: G_neg=V^T.A, mean sq> NW=%d", NW); });
+  KGE_LAUNCH_NAMED(c, name, (k_fused_neg<NW, FLAT>), grid, kThreadsF, smem, m[0], m[1], m[2], m[3], g);
   return launch_error();
 }
 template <int NW>
@@ -914,6 +1037,11 @@ int launch_width(const LaunchCtx& c, bool P, int grid, size_t smem, const CUtens
 }  // namespace
 
 int fused_prefetch_slots(const StepParams& p, int mode) { return geometry(p, mode, true).pf_slots; }
+
+FusedHilo fused_hilo(const StepParams& p) {
+  // k_fused<P>'s GEMM1 width does not depend on prefetch; k_fused<N> is 256 wide only without it
+  return FusedHilo{!k_reg_a(geometry(p, 0, false).N1), !k_reg_a(neg_chunk_width(p.D, false))};
+}
 
 int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int mode, const float* wt, float* dumpS,
                  float* dumpV, const TableView* ent, const long long* neg_ids, const FusedPrefetch* pf) {
@@ -935,7 +1063,11 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
     g.pf_neg_ids = pf->neg_ids; g.pf_nc = pf->nc; g.pf_bn = pf->bn;
     g.xtab = *ent;
   }
-  g.VhiT = w.VhiT; g.VloT = w.VloT; g.colpart = w.colpart; g.ncolpart = (p.Cs + kTileM - 1) / kTileM;
+  // the coefficients go over as fp32, or as hi/lo when k_fused<N> runs 256 columns wide (both launches see the same
+  // prefetch decision, so P writes what N reads)
+  if (k_reg_a(geometry(p, 1, pf != nullptr && ent != nullptr).N1)) g.VT = w.VT;
+  else { g.VhiT = w.VhiT; g.VloT = w.VloT; }
+  g.colpart = w.colpart; g.ncolpart = (p.Cs + kTileM - 1) / kTileM;
   g.dumpV = dumpV;
   const size_t smem = q.ringBytes + 1024;
   const int mtiles = (g.Rx + kTileM - 1) / kTileM;
@@ -951,7 +1083,8 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
     // GEMM2 contracts over the negatives: its operand is the transposed slab copy of Bn
     const long long rowsX = (long long)p.C * p.Cs * g.nblkD, rowsY = (long long)p.C * p.Ns * g.nblkD;
     const long long rowsYT = (long long)p.C * slab_blocks(p.Ns) * p.D;
-    if (tc_make_map(&m[0], w.Ahi, rowsX, 32, kTileM) || tc_make_map(&m[1], w.Alo, rowsX, 32, kTileM) ||
+    const bool ra = k_reg_a(g.N1);
+    if (tc_make_map(&m[0], ra ? w.Af : w.Ahi, rowsX, 32, kTileM) || tc_make_map(&m[1], ra ? w.Af : w.Alo, rowsX, 32, kTileM) ||
         tc_make_map(&m[2], w.Bhi, rowsY, 32, g.N1) || tc_make_map(&m[3], w.Blo, rowsY, 32, g.N1) ||
         tc_make_map(&m[4], w.BhiT, rowsYT, 32, g.N2) || tc_make_map(&m[5], w.BloT, rowsYT, 32, g.N2))
       return KGE_ERR_CUDA;
@@ -964,9 +1097,10 @@ int fused_launch(const LaunchCtx& c, const StepParams& p, const StepWs& w, int m
   if (w.BnRaw) g.xraw = w.BnRaw;
   g.gsn = w.gsn;
   g.out = w.Bn;
-  // A operand: V^T slabs [C][Cs/32][Ns][32]; B operand: A^T slabs [C][Cs/32][D][32]; K = i
+  // A operand: the fp32 V^T slab [C][Cs/32][Ns][32]; B operand: A^T slabs [C][Cs/32][D][32]; K = i
   const long long rowsV = (long long)p.C * slab_blocks(p.Cs) * p.Ns, rowsA = (long long)p.C * slab_blocks(p.Cs) * p.D;
-  if (tc_make_map(&m[0], w.VhiT, rowsV, 32, kTileM) || tc_make_map(&m[1], w.VloT, rowsV, 32, kTileM) ||
+  const bool rv = k_reg_a(g.N1);
+  if (tc_make_map(&m[0], rv ? w.VT : w.VhiT, rowsV, 32, kTileM) || tc_make_map(&m[1], rv ? w.VT : w.VloT, rowsV, 32, kTileM) ||
       tc_make_map(&m[2], w.AhiT, rowsA, 32, g.N1) || tc_make_map(&m[3], w.AloT, rowsA, 32, g.N1))
     return KGE_ERR_CUDA;
   return launch_width(c, false, grid, smem, m, g);

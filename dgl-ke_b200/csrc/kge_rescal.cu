@@ -60,11 +60,12 @@ __global__ void __launch_bounds__(kBlock) k_rescal_fwd(StepParams p, const float
     pos += sh[k] * sMt[k];
     if (want_a) {
       const float av = p.neg_head ? sMt[k] : sMh[k];
-      if (w.Ahi) {
+      if (w.Ahi || w.Af) {
         float hh, ll;
         split_tf32(av, hh, ll);
         const long long o = slab_off(i / p.Cs, slab_blocks(D), p.Cs, (int)(i % p.Cs), k);
-        w.Ahi[o] = hh; w.Alo[o] = ll;
+        if (w.Af) w.Af[o] = av;            // fused step: k_fused<P> splits it
+        else { w.Ahi[o] = hh; w.Alo[o] = ll; }
         if (w.AhiT) {
           const long long ot = slabT_off(i / p.Cs, p.Cs, D, (int)(i % p.Cs), k);
           w.AhiT[ot] = hh; w.AloT[ot] = ll;

@@ -221,8 +221,10 @@ __global__ void __launch_bounds__(kRowBlock, 3) k_prep(StepParams p, TableView e
       const float* t = tail_row(p, ent, b, w, job);
       const float* r = row_ptr(rel, b.rel_ids[job]);
       float pos, a2, reg, nrm;
-      // wgmma engine: A is only consumed as hi/lo operands; fp32 tiles: plain fp32
-      const RowOut ao{w.Ahi ? nullptr : w.A + job * (long long)p.D, w.Ahi, w.Alo, chunk, slab_blocks(p.D), p.Cs, row, st};
+      // wgmma engine: A is only consumed as hi/lo operands; fused step: as fp32 slabs (split by k_fused<P>);
+      // fp32 tiles: plain fp32
+      const RowOut ao{(w.Ahi || w.Af) ? nullptr : w.A + job * (long long)p.D, w.Ahi, w.Alo, chunk, slab_blocks(p.D), p.Cs,
+                      row, st, w.Af};
       edge_forward<MODEL, 1>(p, h, r, t, ao, lane, pos, a2, reg, nrm, true);
       if (lane == 0) {
         w.pos[job] = pos;
