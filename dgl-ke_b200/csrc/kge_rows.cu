@@ -876,21 +876,22 @@ __device__ __forceinline__ void grid_barrier(unsigned int* ctr) {
 // lane (100 per 1600-B row).  Two buffers per warp: the reduction of row i reads one while row i+1 is staged in the other.
 constexpr int kRedRowFloats = 512;
 struct RedStage {
-  float* buf[2];
+  float* buf;           // the warp's two buffers of kRedRowFloats, back to back; null: per-lane red.add instead
   unsigned n;           // rows issued by this warp
 };
+__device__ __forceinline__ float* red_stage_buf(const RedStage& r) { return r.buf + (r.n & 1u) * kRedRowFloats; }
 __device__ __forceinline__ float* red_stage_acquire(RedStage& r, int lane) {
   // the bulk group issued two rows ago read this buffer: all but the newest group must have finished reading
   if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
   __syncwarp();
-  return r.buf[r.n & 1u];
+  return red_stage_buf(r);
 }
 __device__ __forceinline__ void red_stage_issue(RedStage& r, float* dst, int dim, int lane) {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> visible to the async proxy
   __syncwarp();
   if (lane == 0) {
     asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
-                 :: "l"(dst), "r"((unsigned)__cvta_generic_to_shared(r.buf[r.n & 1u])), "r"((unsigned)dim * 4u) : "memory");
+                 :: "l"(dst), "r"((unsigned)__cvta_generic_to_shared(red_stage_buf(r))), "r"((unsigned)dim * 4u) : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
   }
   ++r.n;
@@ -901,17 +902,31 @@ __device__ __forceinline__ void red_stage_drain(int lane) {
 }
 __device__ __forceinline__ void st_shared4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
 
+// state_sum[id] += gs of a row with a unique index, by lane 0; returns the new state in every lane.  On one GPU lane 0
+// loaded the old value st_old together with the row; across GPUs the add is a system-scope atomic, because other GPUs
+// may add to the same state.
+__device__ __forceinline__ float upd_state(float* st, float st_old, float gs, bool sharded, int lane) {
+  float s_new = 0.f;
+  if (lane == 0) {
+    if (sharded) s_new = atomicAdd_system(st, gs) + gs;
+    else { s_new = st_old + gs; *st = s_new; }
+  }
+  return __shfl_sync(0xffffffffu, s_new, 0);
+}
+
+// id = node_ids[u], loaded by the caller one job ahead.  On one GPU the state scalar is loaded together with the row: its
+// address depends only on the id, so the node costs one memory round trip before its stores.
 __device__ __forceinline__ void upd_node(const StepParams& p, const TableView& ent, const BatchView& b, const StepWs& w,
-                                         long long u, int lane, RedStage* rs) {
-  const long long id = b.node_ids[u];
+                                         long long u, long long id, int lane, RedStage& rs) {
   float* row = row_ptr(ent, id);
   float* ng = w.NG + u * (long long)p.D;
-  const float* nc = node_row(p, ent, b, w, u);      // the traced copy of the row (what the reference regularises)
+  const float* nc = p.use_nc ? (w.NC + u * (long long)p.D) : row;   // the traced copy of the row (node_row)
   const int nv = p.D >> 2;
   const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
   const bool sharded = ent.n_shards > 1;
   const bool reg_on = (p.reg_coef > 0.f && p.reg_norm > 0);
   float* st = state_ptr(ent, id);
+  const float st_old = (!sharded && lane == 0) ? *st : 0.f;
   if (nv <= 4 * kWarp) {
     // D <= 512: all of the row's loads (NG and the traced copy) are issued before any arithmetic, and the sums stay in
     // registers for the second half -- one trip through memory and 8 independent 16-byte loads in flight per lane
@@ -934,15 +949,9 @@ __device__ __forceinline__ void upd_node(const StepParams& p, const TableView& e
       reg = warp_sum(reg);
       if (lane == 0) w.regp[p.B + p.Nn + u] = reg;
     }
-    float* st = state_ptr(ent, id);
-    float s_new = 0.f;
-    if (lane == 0) {
-      if (sharded) s_new = atomicAdd_system(st, gs) + gs;   // remote-safe: other GPUs may add to the same state
-      else { s_new = *st + gs; *st = s_new; }
-    }
-    s_new = __shfl_sync(0xffffffffu, s_new, 0);
+    const float s_new = upd_state(st, st_old, gs, sharded, lane);
     const float nlr_std = -p.lr / (sqrtf(s_new) + 1e-10f);
-    float* stage = (sharded && rs) ? red_stage_acquire(*rs, lane) : nullptr;
+    float* stage = (sharded && rs.buf) ? red_stage_acquire(rs, lane) : nullptr;
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int v = lane + kWarp * q;
@@ -953,7 +962,7 @@ __device__ __forceinline__ void upd_node(const StepParams& p, const TableView& e
         st4(ng + 4 * v, z);
       }
     }
-    if (stage) red_stage_issue(*rs, row, p.D, lane);
+    if (stage) red_stage_issue(rs, row, p.D, lane);
     return;
   }
   // pass 1: g = NG + reg'(x), mean(g^2)
@@ -969,12 +978,7 @@ __device__ __forceinline__ void upd_node(const StepParams& p, const TableView& e
     reg = warp_sum(reg);
     if (lane == 0) w.regp[p.B + p.Nn + u] = reg;
   }
-  float s_new = 0.f;
-  if (lane == 0) {
-    if (sharded) s_new = atomicAdd_system(st, gs) + gs;   // remote-safe: other GPUs may add to the same state
-    else { s_new = *st + gs; *st = s_new; }
-  }
-  s_new = __shfl_sync(0xffffffffu, s_new, 0);
+  const float s_new = upd_state(st, st_old, gs, sharded, lane);
   const float stdv = sqrtf(s_new) + 1e-10f;
   const float nlr_std = -p.lr / stdv;
   // pass 2: emb[id] += -lr * g / std.  Indices are unique, so on one GPU the new row is (traced copy + step);
@@ -989,22 +993,47 @@ __device__ __forceinline__ void upd_node(const StepParams& p, const TableView& e
   }
 }
 
-// dense per-relation Adagrad (unique rows): summing the occurrences first is the same math as
-// ExternalEmbedding.update, every occurrence is scaled by the same final state (tensor_models.py:352-361)
-__device__ __forceinline__ void upd_rel_dense(const TableView& rel, float* rg, float* rgs, long long r, float lr, int lane) {
-  const float gs = rgs[r];
-  if (gs == 0.f) return;           // relation not touched this step
-  float* st = state_ptr(rel, r);
+// state_sum[r] += gs by lane 0, then the relation's sum is re-zeroed once every lane has read it
+__device__ __forceinline__ float upd_rel_state(float* st, float st_old, float gs, float* gs_src, int lane) {
   float s_new = 0.f;
-  if (lane == 0) { s_new = *st + gs; *st = s_new; }
+  if (lane == 0) { s_new = st_old + gs; *st = s_new; }
   s_new = __shfl_sync(0xffffffffu, s_new, 0);
   __syncwarp();
-  if (lane == 0) rgs[r] = 0.f;
-  const float stdv = sqrtf(s_new) + 1e-10f;
+  if (lane == 0) *gs_src = 0.f;
+  return s_new;
+}
+// dense per-relation Adagrad (unique rows): summing the occurrences first is the same math as
+// ExternalEmbedding.update, every occurrence is scaled by the same final state (tensor_models.py:352-361).
+// Up to 512 columns, the sum, the state and both rows are loaded at once: one memory round trip per relation.
+__device__ __forceinline__ void upd_rel_dense(const TableView& rel, float* rg, float* rgs, long long r, float lr, int lane) {
+  float* st = state_ptr(rel, r);
   float* row = row_ptr(rel, r);
   float* g = rg + r * (long long)rel.dim;
+  const int nv = rel.dim >> 2;
   const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int v = lane; v < (rel.dim >> 2); v += kWarp) {
+  const float gs = rgs[r], st_old = (lane == 0) ? *st : 0.f;
+  if (nv <= 4 * kWarp) {
+    float4 x[4], e[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int v = lane + kWarp * q;
+      x[q] = (v < nv) ? ld4(g + 4 * v) : z;
+      e[q] = (v < nv) ? ld4(row + 4 * v) : z;
+    }
+    if (gs == 0.f) return;         // relation not touched this step
+    const float s_new = upd_rel_state(st, st_old, gs, rgs + r, lane);
+    const float stdv = sqrtf(s_new) + 1e-10f;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int v = lane + kWarp * q;
+      if (v < nv) { st4(row + 4 * v, f4_fma(x[q], -lr / stdv, e[q])); st4(g + 4 * v, z); }
+    }
+    return;
+  }
+  if (gs == 0.f) return;
+  const float s_new = upd_rel_state(st, st_old, gs, rgs + r, lane);
+  const float stdv = sqrtf(s_new) + 1e-10f;
+  for (int v = lane; v < nv; v += kWarp) {
     float4 x = ld4(g + 4 * v), e = ld4(row + 4 * v);
     st4(row + 4 * v, f4_fma(x, -lr / stdv, e));
     st4(g + 4 * v, z);
@@ -1012,7 +1041,7 @@ __device__ __forceinline__ void upd_rel_dense(const TableView& rel, float* rg, f
 }
 
 __device__ __forceinline__ void apply_row(const TableView& t, long long id, const float* g, int dim, float lr, int lane,
-                                          RedStage* rs = nullptr) {
+                                          RedStage& rs) {
   float* row = row_ptr(t, id);
   const int nv = dim >> 2;
   if (nv <= 4 * kWarp && (dim & 3) == 0) {
@@ -1024,14 +1053,14 @@ __device__ __forceinline__ void apply_row(const TableView& t, long long id, cons
       x[q] = (v < nv) ? ld4(g + 4 * v) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
     const float nlr_std = -lr / (sqrtf(*state_ptr(t, id)) + 1e-10f);
-    if (rs) {
-      float* stage = red_stage_acquire(*rs, lane);
+    if (rs.buf) {
+      float* stage = red_stage_acquire(rs, lane);
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const int v = lane + kWarp * q;
         if (v < nv) st_shared4(stage + 4 * v, f4_scale(x[q], nlr_std));
       }
-      red_stage_issue(*rs, row, dim, lane);
+      red_stage_issue(rs, row, dim, lane);
       return;
     }
 #pragma unroll
@@ -1053,58 +1082,74 @@ __device__ __forceinline__ void apply_row(const TableView& t, long long id, cons
 __device__ void reduce_log_part(const StepParams& p, const StepWs& w, long long nreg, const float* wbar, float* log4,
                                 int bid, int nb);
 
-__global__ void __launch_bounds__(kRowBlock, 4) k_update(UpdArgs a) {
+// Two CTAs per SM (16 warps): the kernel takes 100 registers and spills none.  Held to 64 registers (4 CTAs) it spilled
+// its loop state and the bulk-reduction staging state to local memory inside the row loops, and at 80 (3 CTAs) it still
+// spilled; on an H100 both were slower (DESIGN.md section 4).
+__global__ void __launch_bounds__(kRowBlock, 2) k_update(UpdArgs a) {
   __shared__ __align__(128) float red_stage[kWarpsPerBlock][2][kRedRowFloats];
   const StepParams& p = a.p;
   const StepWs& w = a.w;
   const int lane = threadIdx.x & 31;
-  RedStage rstage{{red_stage[threadIdx.x >> 5][0], red_stage[threadIdx.x >> 5][1]}, 0u};
-  RedStage* rs = a.bulk_red ? &rstage : nullptr;
-  const long long warp0 = (long long)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-  const long long nwarps = (long long)gridDim.x * kWarpsPerBlock;
+  RedStage rs{a.bulk_red ? red_stage[threadIdx.x >> 5][0] : nullptr, 0u};
+  RedStage per_lane{nullptr, 0u};
+  const int warp0 = (int)blockIdx.x * kWarpsPerBlock + (int)(threadIdx.x >> 5);
+  const int nwarps = (int)gridDim.x * kWarpsPerBlock;
   const bool rel_edge = !p.rel_deferred && !p.rel_dense;      // relation entry handled per edge, here
-  for (int phase = a.phase_lo; phase <= a.phase_hi; ++phase) {
-    if (phase == 1) {
-      const long long nrel = (p.rel_dense && !p.rel_deferred) ? a.rel.num_rows : 0;
-      const long long U = node_count(p);
-      for (long long j = warp0; j < U + nrel; j += nwarps) {
-        if (j < U) upd_node(p, a.ent, a.b, w, j, lane, rs);
-        else upd_rel_dense(a.rel, w.rg, w.rgs, j - U, p.lr, lane);
-      }
-    } else if (phase == 2) {
-      if (p.fused) {
-        // mean(G_neg^2) came out of the fused kernel's epilogue: one scalar atomic per negative row
-        const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
-        for (long long j = t0; j < p.Nn; j += nt) table_atomic_add(a.ent, state_ptr(a.ent, a.b.neg_ids[j]), w.gsn[j]);
-      } else {
-        for (long long j = warp0; j < p.Nn; j += nwarps) {
-          const float* g = w.Bn + j * (long long)p.D;
-          float gs = 0.f;
-          for (int v = lane; v < (p.D >> 2); v += kWarp) { float4 x = ld4(g + 4 * v); gs += f4_dot(x, x); }
-          gs = warp_sum(gs);
-          if (lane == 0) table_atomic_add(a.ent, state_ptr(a.ent, a.b.neg_ids[j]), gs / (float)p.D);
-        }
-      }
-      if (rel_edge) {
-        const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
-        for (long long i = t0; i < p.B; i += nt) table_atomic_add(a.rel, state_ptr(a.rel, a.b.rel_ids[i]), w.gsr[i]);
-      }
+  // phases a.phase_lo..a.phase_hi as straight-line code: a phase counter live across all three cost a spill
+  if (a.phase_lo <= 1) {
+    const long long nrel = (p.rel_dense && !p.rel_deferred) ? a.rel.num_rows : 0;
+    const long long U = node_count(p);
+    // a node's id is loaded one job ahead, before the stores of the job in hand: its row loads wait on no index load
+    long long id = (warp0 < U) ? a.b.node_ids[warp0] : 0;
+    for (long long j = warp0; j < U + nrel; j += nwarps) {
+      const long long cur = id;
+      if (j + nwarps < U) id = a.b.node_ids[j + nwarps];
+      if (j < U) upd_node(p, a.ent, a.b, w, j, cur, lane, rs);
+      else upd_rel_dense(a.rel, w.rg, w.rgs, j - U, p.lr, lane);
+    }
+    if (a.phase_hi > 1) grid_barrier(w.sync_ctr + 0);
+  }
+  if (a.phase_lo <= 2 && a.phase_hi >= 2) {
+    if (p.fused) {
+      // mean(G_neg^2) came out of the fused kernel's epilogue: one scalar atomic per negative row
+      const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+      for (long long j = t0; j < p.Nn; j += nt) table_atomic_add(a.ent, state_ptr(a.ent, a.b.neg_ids[j]), w.gsn[j]);
     } else {
-      const long long nr = rel_edge ? p.B : 0;
-      for (long long j = warp0; j < p.Nn + nr; j += nwarps) {
-        if (j < p.Nn) apply_row(a.ent, a.b.neg_ids[j], w.Bn + j * (long long)p.D, p.D, p.lr, lane, rs);
-        else apply_row(a.rel, a.b.rel_ids[j - p.Nn], w.GR + (j - p.Nn) * (long long)p.Dr, p.Dr, p.lr, lane);
-      }
-      if (a.log4) {
-        const int nb = gridDim.x < 64 ? gridDim.x : 64;
-        const bool reg_on = (p.reg_coef > 0.f && p.reg_norm > 0);
-        if ((int)blockIdx.x < nb)
-          reduce_log_part(p, w, reg_on ? (p.B + p.Nn + node_count(p)) : 0, a.wt ? w.wbar : nullptr, a.log4, blockIdx.x, nb);
+      for (long long j = warp0; j < p.Nn; j += nwarps) {
+        const float* g = w.Bn + j * (long long)p.D;
+        float gs = 0.f;
+        for (int v = lane; v < (p.D >> 2); v += kWarp) { float4 x = ld4(g + 4 * v); gs += f4_dot(x, x); }
+        gs = warp_sum(gs);
+        if (lane == 0) table_atomic_add(a.ent, state_ptr(a.ent, a.b.neg_ids[j]), gs / (float)p.D);
       }
     }
-    if (phase < a.phase_hi) grid_barrier(w.sync_ctr + (phase - 1));
+    if (rel_edge) {
+      const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+      for (long long i = t0; i < p.B; i += nt) table_atomic_add(a.rel, state_ptr(a.rel, a.b.rel_ids[i]), w.gsr[i]);
+    }
+    if (a.phase_hi > 2) grid_barrier(w.sync_ctr + 1);
   }
-  if (rs) red_stage_drain(lane);        // every bulk reduction of this warp has landed
+  if (a.phase_hi >= 3) {
+    const long long nr = rel_edge ? p.B : 0;
+    // the row's index, one job ahead (as in phase 1): the state and gradient loads of a job wait on no index load
+    auto job_id = [&](long long j) { return j < p.Nn ? a.b.neg_ids[j] : (j < p.Nn + nr ? a.b.rel_ids[j - p.Nn] : 0); };
+    long long id = job_id(warp0);
+    for (long long j = warp0; j < p.Nn + nr; j += nwarps) {
+      const long long cur = id;
+      id = job_id(j + nwarps);
+      if (j < p.Nn) apply_row(a.ent, cur, w.Bn + j * (long long)p.D, p.D, p.lr, lane, rs);
+      else apply_row(a.rel, cur, w.GR + (j - p.Nn) * (long long)p.Dr, p.Dr, p.lr, lane, per_lane);
+    }
+    if (a.log4) {
+      // on the last CTAs: warps are handed jobs in index order, so those have the fewest rows to apply
+      const int nb = gridDim.x < 64 ? gridDim.x : 64;
+      const int bid = (int)blockIdx.x - ((int)gridDim.x - nb);
+      const bool reg_on = (p.reg_coef > 0.f && p.reg_norm > 0);
+      if (bid >= 0)
+        reduce_log_part(p, w, reg_on ? (p.B + p.Nn + node_count(p)) : 0, a.wt ? w.wbar : nullptr, a.log4, bid, nb);
+    }
+  }
+  if (rs.buf) red_stage_drain(lane);        // every bulk reduction of this warp has landed
   if (a.phase_hi > a.phase_lo) {
     // leave the barrier counters at zero for the next launch: the last CTA to get here resets them
     __syncthreads();
@@ -1179,7 +1224,8 @@ __global__ void __launch_bounds__(kRowBlock) k_apply(TableView t, const long lon
                                                       const float* __restrict__ grad, long long n, int dim, float lr) {
   const long long j = (long long)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
   if (j >= n) return;
-  apply_row(t, idx[j], grad + j * (long long)dim, dim, lr, threadIdx.x & 31);
+  RedStage per_lane{nullptr, 0u};
+  apply_row(t, idx[j], grad + j * (long long)dim, dim, lr, threadIdx.x & 31, per_lane);
 }
 
 // ---- multi-GPU relation path: per-edge gradients -> dense per-relation sums (all-reduced by the host
