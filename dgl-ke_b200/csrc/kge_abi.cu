@@ -570,6 +570,46 @@ KGE_API int kge_score_neg(kge_handle_t h, const kge_step_cfg_t* cfg, const float
   return KGE_OK;
 }
 
+KGE_API int kge_rank_count(kge_handle_t h, const float* S, int64_t ld, int64_t Q, int64_t N, const float* pos,
+                           int64_t base, const int64_t* cand, int64_t chunk, const int64_t* kept, const int64_t* rel,
+                           const kge_filter_t* filter, int64_t* cnt, void* stream) {
+  if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
+  if (Q < 0 || N < 0 || ld < N) return fail(KGE_ERR_INVALID_ARG, "bad tile shape Q=%lld N=%lld ld=%lld", (long long)Q,
+                                            (long long)N, (long long)ld);
+  if (Q == 0 || N == 0) return KGE_OK;
+  if (!S || !pos || !cnt) return fail(KGE_ERR_INVALID_ARG, "null pointer");
+  if (cand && chunk <= 0) return fail(KGE_ERR_INVALID_ARG, "chunk must be positive with explicit candidates");
+  if (!cand && base < 0) return fail(KGE_ERR_INVALID_ARG, "base < 0");
+  const bool filt = filter && filter->n_keys > 0;
+  if (filt && (!filter->keys || !filter->vals || !kept || !rel || filter->n_rel <= 0))
+    return fail(KGE_ERR_INVALID_ARG, "filter needs keys, vals, kept, rel and n_rel > 0");
+  if (Q * ((N + 1023) / 1024) > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARG, "tile too large");
+  RankParams p{};
+  p.S = S; p.ld = ld; p.Q = Q; p.N = N; p.pos = pos;
+  p.base = base; p.cand = (const long long*)cand; p.chunk = chunk;
+  p.kept = (const long long*)kept; p.rel = (const long long*)rel;
+  p.keys = filt ? (const long long*)filter->keys : nullptr;
+  p.vals = filt ? (const int*)filter->vals : nullptr;
+  p.n_keys = filt ? filter->n_keys : 0;
+  p.n_rel = filt ? filter->n_rel : 1;
+  p.cnt = (long long*)cnt;
+  DeviceGuard g(h->device);
+  launch_rank_count(lctx(h, stream), p);
+  KGE_CUDA_OK(cudaGetLastError());
+  return KGE_OK;
+}
+
+KGE_API int kge_rank_finish(kge_handle_t h, const int64_t* cnt, int64_t Q, int64_t* rank_out, double* acc, void* stream) {
+  if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
+  if (Q < 0) return fail(KGE_ERR_INVALID_ARG, "Q < 0");
+  if (Q == 0) return KGE_OK;
+  if (!cnt || !acc) return fail(KGE_ERR_INVALID_ARG, "null pointer");
+  DeviceGuard g(h->device);
+  launch_rank_finish(lctx(h, stream), (const long long*)cnt, Q, (long long*)rank_out, acc);
+  KGE_CUDA_OK(cudaGetLastError());
+  return KGE_OK;
+}
+
 KGE_API int kge_loss_grad(kge_handle_t h, const kge_step_cfg_t* cfg, const float* pos, const float* neg, const float* wt,
                   float* dpos, float* dneg, float* log4, void* stream) {
   if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");

@@ -424,6 +424,24 @@ void launch_negdeg_mask_scores(const LaunchCtx&, const StepParams&, const StepWs
 void launch_negdeg_mask_coef(const LaunchCtx&, const StepParams&, const StepWs&);
 void launch_negdeg_scatter(const LaunchCtx&, const StepParams&, const TableView& ent, const BatchView&, const StepWs&);
 
+// filtered ranking of evaluation queries over one score tile (kge_eval.cu)
+struct RankParams {
+  const float* S;               // [Q, ld] score tile, N columns used
+  long long ld, Q, N;
+  const float* pos;             // [Q]
+  long long base;               // range ids: column j is entity base + j (cand == null)
+  const long long* cand;        // explicit ids: [Q / chunk, N], query q reads row q / chunk
+  long long chunk;
+  const long long* kept;        // [Q] the query's kept-side entity and its relation: key = kept * n_rel + rel
+  const long long* rel;
+  const long long* keys;        // [n_keys] sorted, or null: no filter
+  const int* vals;              // [n_keys] sorted and distinct within each key
+  long long n_keys, n_rel;
+  long long* cnt;               // [Q]
+};
+void launch_rank_count(const LaunchCtx&, const RankParams&);
+void launch_rank_finish(const LaunchCtx&, const long long* cnt, long long Q, long long* rank_out, double* acc);
+
 // RESCAL-specific row kernels (kge_rescal.cu)
 int launch_rescal_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
                        const BatchView&, const StepWs&);

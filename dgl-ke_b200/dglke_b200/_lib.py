@@ -21,7 +21,8 @@ EXPORTS = ["kge_abi_version", "kge_last_error", "kge_create", "kge_destroy", "kg
            "kge_set_engine", "kge_set_fused", "kge_debug_set_dump", "kge_profile_enable", "kge_profile_read", "kge_set_relation_mode", "kge_set_relation_buffers",
            "kge_rel_grad_dense", "kge_rel_apply_dense", "kge_device_alloc", "kge_device_free", "kge_ipc_export",
            "kge_ipc_open", "kge_shard_alloc", "kge_shard_import", "kge_shard_free",
-           "kge_set_next_batch", "kge_sampler_create", "kge_sampler_destroy", "kge_sampler_sample"]
+           "kge_set_next_batch", "kge_sampler_create", "kge_sampler_destroy", "kge_sampler_sample",
+           "kge_rank_count", "kge_rank_finish"]
 
 
 class KgeError(RuntimeError):
@@ -55,6 +56,10 @@ class Batch(C.Structure):
                 ("tail_local", C.c_void_p), ("rel_ids", C.c_void_p), ("neg_ids", C.c_void_p),
                 ("edge_weight", C.c_void_p), ("n_nodes_dev", C.c_void_p), ("head_ids", C.c_void_p),
                 ("tail_ids", C.c_void_p)]
+
+
+class Filter(C.Structure):
+    _fields_ = [("keys", C.c_void_p), ("vals", C.c_void_p), ("n_keys", C.c_int64), ("n_rel", C.c_int64)]
 
 
 _lib = None
@@ -110,6 +115,8 @@ def load_library():
     lib.kge_sampler_create.argtypes = [vp, vp, vp, vp, i64, i64, i64, i32, C.c_uint64, P(vp)]
     lib.kge_sampler_destroy.argtypes = [vp]
     lib.kge_sampler_sample.argtypes = [vp, i64, P(Batch), P(i32), vp]
+    lib.kge_rank_count.argtypes = [vp, vp, i64, i64, i64, vp, i64, vp, i64, vp, vp, P(Filter), vp, vp]
+    lib.kge_rank_finish.argtypes = [vp, vp, i64, vp, vp, vp]
     missing = [name for name in EXPORTS if not hasattr(lib, name)]
     if missing:
         raise KgeError("libkge_b200.so at %s lacks symbols %s (stale build?)" % (LIB_PATH, missing))

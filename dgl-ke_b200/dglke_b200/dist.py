@@ -189,6 +189,21 @@ class ShardedTrainer:
         self._log_host.copy_(out, non_blocking=True)
         return self._log_host
 
+    def evaluate(self, split, batch_size, neg_sample_size=-1, block_rows=None, seed=0):
+        """Filtered ranking of this rank's slice of `split` (an evaluate.EvalSplit) over the sharded entity table.
+        Returns (this rank's six sums, the sums all-reduced over the group), float64 CPU tensors; see
+        evaluate.metrics_from_sums.  The evaluation runs on a handle of its own, so rows a pipelined step staged for the
+        next step (kge_set_next_batch) stay staged and valid: evaluation does not write the tables."""
+        from .evaluate import Evaluator
+        ev = Evaluator(self.hp, self.ent, self.rel, self.device, block_rows=block_rows, seed=seed * 1000003 + self.rank)
+        try:
+            local = ev.run(split, batch_size, neg_sample_size).clone()
+        finally:
+            ev.close()
+        pooled = local.clone()
+        dist.all_reduce(pooled, op=dist.ReduceOp.SUM, group=self.group)
+        return local.cpu(), pooled.cpu()
+
     def sync(self):
         torch.cuda.current_stream(self.device).synchronize()
 

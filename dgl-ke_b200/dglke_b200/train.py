@@ -26,6 +26,7 @@ from .utils import ArgParser, get_compatible_batch_size, save_model, prepare_sav
 from .general_models import KEModel
 from .graph import SyntheticSampler, TripleSampler, TripleFilter, eval_batches, NegGraph
 from .sampler import DeviceSampler
+from .evaluate import EvalSplit, Evaluator, FilterIndex, check_eval_flags, metrics_from_sums, select_eval_edges
 
 # (entities, relations, training edges): docs/source/benchmarks.rst dataset table
 BUILTIN_SHAPES = {
@@ -132,14 +133,22 @@ def train(args, model, train_sampler, valid_batches=None, rank=0, barrier=None):
 def test(args, model, batches, rank=0, mode="Test"):
     """train_pytorch.py:199-253 (non-wikikg90M branch): average MRR / MR / HITS@k over head and tail ranking."""
     gpu_id = args.gpu[rank % len(args.gpu)]
-    logs = []
-    with th.no_grad():
-        for pos_g, neg_g in batches:
-            model.forward_test(pos_g, neg_g, logs, gpu_id)
-    metrics = {}
-    if logs:
-        for m in logs[0].keys():
-            metrics[m] = sum(l[m] for l in logs) / len(logs)
+    if isinstance(batches, EvalSplit):
+        # --neg_sample_size_eval > 0: chunked sampled candidates, ranks counted on the GPU (dglke_b200.evaluate)
+        ev = Evaluator(model.hyper, model.entity_emb.table(), model.relation_emb.table(), model.device)
+        try:
+            metrics = metrics_from_sums(ev.run(batches, args.batch_size_eval, args.neg_sample_size_eval).cpu())
+        finally:
+            ev.close()
+    else:
+        logs = []
+        with th.no_grad():
+            for pos_g, neg_g in batches:
+                model.forward_test(pos_g, neg_g, logs, gpu_id)
+        metrics = {}
+        if logs:
+            for m in logs[0].keys():
+                metrics[m] = sum(l[m] for l in logs) / len(logs)
     for k, v in metrics.items():
         print("[{}]{} average {}: {}".format(rank, mode, k, v))
     return metrics
@@ -149,6 +158,7 @@ def main(argv=None):
     args = ArgParser().parse_args(argv)
     if args.gpu[0] < 0:
         raise SystemExit("dglke_b200 needs --gpu: the hot path is an H100 CUDA library without a CPU fallback")
+    check_eval_flags(args)
     prepare_save_path(args)
     args.eval_filter = not args.no_eval_filter
     args.strict_rel_part = args.soft_rel_part = False
@@ -160,8 +170,16 @@ def main(argv=None):
         print("|Train|: {}  entities: {}  relations: {}".format(len(tr[0]), n_ent, n_rel))
     if tr is not None and len(tr) == 4 and not args.has_edge_importance:
         tr = tr[:3]
+    # filtered evaluation (the default; --no_eval_filter turns it off): candidates that form a triple of train / valid /
+    # test are left out of the ranking (EvalDataset builds its graph from all three splits, sampler.py:604-640)
+    known_triples = None
+    if args.eval_filter and dataset is not None and (va is not None or te is not None):
+        allt = [x for x in (tr, va, te) if x is not None]
+        known_triples = tuple(np.concatenate([x[k] for x in allt]) for k in range(3))
+    va, te = (None if s is None else select_eval_edges(s, args.eval_percent, seed=k) for k, s in enumerate((va, te)))
     if len(args.gpu) > 1:
-        return train_multi_gpu(args, n_ent, n_rel, tr if tr is not None else synthetic_edges(n_ent, n_rel, n_edges))
+        return train_multi_gpu(args, n_ent, n_rel, tr if tr is not None else synthetic_edges(n_ent, n_rel, n_edges),
+                               va, te, known_triples)
     th.cuda.set_device(args.gpu[0])
     model = KEModel(args, args.model_name, n_ent, n_rel, args.hidden_dim, args.gamma,
                     double_entity_emb=args.double_ent, double_relation_emb=args.double_rel)
@@ -176,14 +194,17 @@ def main(argv=None):
         sampler = DeviceGraphSampler(edges[0], edges[1], edges[2], n_ent, args.batch_size, args.neg_sample_size, seed=0,
                                      device=args.gpu[0])
 
-    # filtered evaluation (the default; --no_eval_filter turns it off): candidates that form a triple of train / valid /
-    # test are left out of the ranking (EvalDataset builds its graph from all three splits, sampler.py:604-640)
-    known = None
-    if args.eval_filter and dataset is not None and (va is not None or te is not None):
-        allt = [x for x in (tr, va, te) if x is not None]
-        known = TripleFilter(*(np.concatenate([x[k] for x in allt]) for k in range(3)), n_rel)
+    known = index = None
+    if known_triples is not None and args.neg_sample_size_eval > 0:
+        index = FilterIndex.build(*known_triples, n_rel)
+    elif known_triples is not None:
+        known = TripleFilter(*known_triples, n_rel)
 
     def split_batches(split):
+        if args.neg_sample_size_eval > 0:
+            es = EvalSplit(split, model.device, index)
+            return lambda: es
+
         def gen():
             for neg_head in (True, False):
                 yield from eval_batches(split[0], split[1], split[2], n_ent, args.batch_size_eval, neg_head, known=known)
@@ -206,8 +227,10 @@ def hyper_from_args(args):
                  margin=args.margin, pairwise=args.pairwise, neg_deg_sample=args.neg_deg_sample)
 
 
-def _multi_gpu_worker(rank, world, args, n_ent, n_rel, edges, port):
-    """One process per GPU (reference: train.py:298-317 forks one process per GPU over a shared host table)."""
+def _multi_gpu_worker(rank, world, args, n_ent, n_rel, edges, port, valid=None, test=None, index=None):
+    """One process per GPU (reference: train.py:298-317 forks one process per GPU over a shared host table).
+    valid / test: the evaluation splits (after --eval_percent); index: evaluate.FilterIndex of the known triples, or None
+    (raw ranks).  Rank r evaluates its slice of each split (evaluate.rank_slice)."""
     import torch.distributed as dist
     from .dist import ShardedTrainer
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
@@ -227,6 +250,8 @@ def _multi_gpu_worker(rank, world, args, n_ent, n_rel, edges, port):
             raise SystemExit("rank %d owns the heads of only %d edges (< batch_size): use KGE_B200_EDGE_PART=random" % (rank, len(perm)))
     sampler = DeviceSampler(edges[0][perm], edges[1][perm], edges[2][perm], n_ent, args.batch_size, args.neg_sample_size,
                             seed=1000 + rank, device=dev.index)
+    vsplit = EvalSplit(valid, dev, index, rank, world) if args.valid and valid is not None else None
+    tsplit = EvalSplit(test, dev, index, rank, world) if args.test and test is not None else None
     start = t0 = time.time()
     logs = []
     # --async_update (tensor_models.py:136-175: the update runs behind the trainer, which may read rows one update old):
@@ -248,8 +273,20 @@ def _multi_gpu_worker(rank, world, args, n_ent, n_rel, edges, port):
             start = time.time()
         if args.force_sync_interval > 0 and (step + 1) % args.force_sync_interval == 0:
             trainer.barrier()                       # train_pytorch.py:157-159
+        if vsplit is not None and (step + 1) % args.eval_interval == 0 and step > 1:
+            # between step k and k+1: a step announced with --async_update keeps the rows staged for it
+            local, _ = trainer.evaluate(vsplit, args.batch_size_eval, args.neg_sample_size_eval)
+            for k, v in metrics_from_sums(local).items():
+                print("[{}]Valid average {}: {}".format(rank, k, v))
     trainer.barrier()
     print("proc {} takes {:.3f} seconds".format(rank, time.time() - t0))
+    if tsplit is not None:
+        _, pooled = trainer.evaluate(tsplit, args.batch_size_eval, args.neg_sample_size_eval)
+        if rank == 0:                               # train.py:357-369: the ranks of every process, pooled
+            print("-------------- Test result --------------")
+            for k, v in metrics_from_sums(pooled).items():
+                print("Test average {} : {}".format(k, v))
+            print("-----------------------------------------")
     if not args.no_save_emb:
         ent = trainer.gather_entity_table()
         if rank == 0:
@@ -261,7 +298,7 @@ def _multi_gpu_worker(rank, world, args, n_ent, n_rel, edges, port):
     dist.destroy_process_group()
 
 
-def train_multi_gpu(args, n_ent, n_rel, edges):
+def train_multi_gpu(args, n_ent, n_rel, edges, valid=None, test=None, known_triples=None):
     import torch.multiprocessing as mp
     world = len(args.gpu)
     if args.has_edge_importance:
@@ -270,7 +307,8 @@ def train_multi_gpu(args, n_ent, n_rel, edges):
         raise SystemExit("--neg_deg_sample is single-GPU only here: it needs an unsharded entity table")
     port = 29400 + os.getpid() % 1000
     edges = tuple(np.ascontiguousarray(e, dtype=np.int64) for e in edges)
-    mp.spawn(_multi_gpu_worker, args=(world, args, n_ent, n_rel, edges, port), nprocs=world, join=True)
+    index = FilterIndex.build(*known_triples, n_rel) if known_triples is not None and (args.valid or args.test) else None
+    mp.spawn(_multi_gpu_worker, args=(world, args, n_ent, n_rel, edges, port, valid, test, index), nprocs=world, join=True)
     return None
 
 

@@ -238,6 +238,33 @@ KGE_API int kge_sampler_destroy(kge_sampler_t s);
  * next-but-one call), n_nodes = -1 and n_nodes_dev set; *neg_head_out = step & 1. */
 KGE_API int kge_sampler_sample(kge_sampler_t s, int64_t step, kge_batch_t* batch_out, int32_t* neg_head_out, void* stream);
 
+/* --- filtered ranking of evaluation queries (KEModel.forward_test's rank, general_models.py:462-485) -----------------
+ *   rank_q = 1 + #{ j : S[q, j] >= pos[q] (IEEE: a NaN never counts) and candidate j is not a known triple of q }
+ * over the score tiles of kge_score_neg, tile by tile, without a [queries, candidates] mask.
+ *
+ * The known triples of one corruption side: keys[i] = kept_entity * n_rel + rel, sorted; vals[i] = the corrupted-side
+ * entity, sorted and distinct within each key (device arrays).  Corrupting heads, the kept side is the tail. */
+typedef struct {
+  const int64_t* keys;
+  const int32_t* vals;
+  int64_t n_keys;
+  int64_t n_rel;
+} kge_filter_t;
+
+/* Adds one score tile's hits to cnt[Q] (int64, zeroed by the caller once per batch of queries).
+ *   S [Q, ld]: N columns used;  pos [Q]: the positives' scores
+ *   kept [Q], rel [Q]: each query's kept-side entity and relation (read only with a filter)
+ *   cand == NULL: column j is entity base + j (a block of rows of one shard);
+ *   cand != NULL: cand [Q / chunk, N] int64 ids, query q ranks against row q / chunk (chunked sampled candidates)
+ *   filter == NULL or filter->n_keys == 0: raw ranks */
+KGE_API int kge_rank_count(kge_handle_t h, const float* S, int64_t ld, int64_t Q, int64_t N, const float* pos,
+                           int64_t base, const int64_t* cand, int64_t chunk, const int64_t* kept, const int64_t* rel,
+                           const kge_filter_t* filter, int64_t* cnt, void* stream);
+/* rank = cnt + 1: written to rank_out [Q] (int64) unless NULL, and {sum 1/r, sum r, #(r<=1), #(r<=3), #(r<=10), Q}
+ * added to acc [6] (device doubles, caller-owned; reduced in a fixed order, so the sums do not depend on timing). */
+KGE_API int kge_rank_finish(kge_handle_t h, const int64_t* cnt, int64_t Q, int64_t* rank_out, double* acc,
+                            void* stream);
+
 /* --- introspection (parity tests read the traced gradients the way the reference exposes
  *     `data.grad` of each trace entry, tensor_models.py:318) ---------------------------------- */
 typedef enum {
