@@ -119,6 +119,7 @@ struct kge_context {
   float* ext_rgs = nullptr;          //   the relation gradients into (all-reduced by the caller, kge_set_relation_buffers)
   float* dump_v = nullptr;           // test hook (kge_debug_set_dump): coefficient matrices of the fused kernel
   Buffer negdeg_ids;                 // --neg_deg_sample: the augmented negative id list [C * (Cs + Ns)] of the last step
+  Buffer topk_ws;                    // kge_topk: the select CTAs' survivors and the per-list bounds
   // kge_set_next_batch: rows of the next step staged by this step's fused kernels
   struct Prefetch {
     bool armed = false;              // a next batch is registered for the coming kge_step_fused_begin
@@ -435,7 +436,7 @@ KGE_API int kge_destroy(kge_handle_t h) {
   if (!h) return KGE_OK;
   DeviceGuard g(h->device);
   cudaDeviceSynchronize();
-  for (Buffer* b : {&h->arena, &h->dev_stage, &h->pin, &h->rel_dense, &h->negdeg_ids, &h->pf.nc[0], &h->pf.nc[1],
+  for (Buffer* b : {&h->arena, &h->dev_stage, &h->pin, &h->rel_dense, &h->negdeg_ids, &h->topk_ws, &h->pf.nc[0], &h->pf.nc[1],
                     &h->pf.bn[0], &h->pf.bn[1]})
     b->release();
   if (h->dev_log4) cudaFree(h->dev_log4);
@@ -606,6 +607,39 @@ KGE_API int kge_rank_finish(kge_handle_t h, const int64_t* cnt, int64_t Q, int64
   if (!cnt || !acc) return fail(KGE_ERR_INVALID_ARG, "null pointer");
   DeviceGuard g(h->device);
   launch_rank_finish(lctx(h, stream), (const long long*)cnt, Q, (long long*)rank_out, acc);
+  KGE_CUDA_OK(cudaGetLastError());
+  return KGE_OK;
+}
+
+KGE_API int kge_topk(kge_handle_t h, const float* S, int64_t ld, int64_t Q, int64_t N, const int64_t* qgroup,
+                     const int64_t* qoff, int64_t cbase, int64_t cstride, int32_t K, int64_t G, float* top_score,
+                     int64_t* top_key, void* stream) {
+  if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
+  if (K > KGE_TOPK_MAX) return fail(KGE_ERR_UNSUPPORTED, "K=%d: kge_topk keeps at most KGE_TOPK_MAX=%d entries per list",
+                                    (int)K, KGE_TOPK_MAX);
+  if (K < 1) return fail(KGE_ERR_INVALID_ARG, "K=%d must be positive", (int)K);
+  if (Q < 0 || N < 0 || ld < N || G < 1) return fail(KGE_ERR_INVALID_ARG, "bad tile shape Q=%lld N=%lld ld=%lld G=%lld",
+                                                    (long long)Q, (long long)N, (long long)ld, (long long)G);
+  if (cbase < 0 || cstride < 1) return fail(KGE_ERR_INVALID_ARG, "cbase=%lld must be >= 0 and cstride=%lld >= 1",
+                                            (long long)cbase, (long long)cstride);
+  if (Q == 0 || N == 0) return KGE_OK;
+  if (!S || !qgroup || !qoff || !top_score || !top_key) return fail(KGE_ERR_INVALID_ARG, "null pointer");
+  if (Q * ((N + kTopkSeg - 1) / kTopkSeg) > 0x7fffffffLL || Q > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARG, "tile too large");
+  DeviceGuard g(h->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const size_t bytes = topk_workspace_bytes(Q, N, K, G);
+  if (h->topk_ws.bytes < bytes) {
+    const int rc = h->topk_ws.resize(bytes, st, "top-K workspace");
+    if (rc) return rc;
+  }
+  TopkParams p{};
+  p.S = S; p.ld = ld; p.Q = Q; p.N = N;
+  p.qgroup = (const long long*)qgroup; p.qoff = (const long long*)qoff;
+  p.cbase = cbase; p.cstride = cstride; p.K = K;
+  p.top_score = top_score; p.top_key = (long long*)top_key;
+  topk_carve(p, h->topk_ws.p);
+  KGE_CUDA_OK(cudaMemsetAsync(p.bound, 0, (size_t)G * sizeof(unsigned), st));
+  launch_topk(lctx(h, stream), p);
   KGE_CUDA_OK(cudaGetLastError());
   return KGE_OK;
 }

@@ -442,6 +442,27 @@ struct RankParams {
 void launch_rank_count(const LaunchCtx&, const RankParams&);
 void launch_rank_finish(const LaunchCtx&, const long long* cnt, long long Q, long long* rank_out, double* acc);
 
+// running top-K lists over one score tile (kge_topk.cu)
+constexpr int kTopkSeg = 4096;            // columns per select CTA
+struct TopkParams {
+  const float* S;               // [Q, ld] score tile, N columns used
+  long long ld, Q, N;
+  const long long* qgroup;      // [Q] list of each row (a list's rows are consecutive)
+  const long long* qoff;        // [Q] key of (q, j) = qoff[q] + (cbase + j) * cstride
+  long long cbase, cstride;
+  int K;
+  float* top_score;             // [G, K] in list order, empty slots -inf / -1
+  long long* top_key;
+  // workspace (topk_carve): the select CTAs' survivors [Q * nseg, K], their counts, the per-list bound [G]
+  float* cs;
+  long long* ck;
+  int* cn;
+  unsigned* bound;
+};
+size_t topk_workspace_bytes(long long Q, long long N, int K, long long G);
+void topk_carve(TopkParams& p, void* ws);
+void launch_topk(const LaunchCtx&, const TopkParams&);
+
 // RESCAL-specific row kernels (kge_rescal.cu)
 int launch_rescal_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
                        const BatchView&, const StepWs&);

@@ -22,7 +22,7 @@ import time
 import numpy as np
 import torch as th
 
-from .utils import ArgParser, get_compatible_batch_size, save_model, prepare_save_path
+from .utils import ArgParser, get_compatible_batch_size, save_model, save_config, prepare_save_path
 from .general_models import KEModel
 from .graph import SyntheticSampler, TripleSampler, TripleFilter, eval_batches, NegGraph
 from .sampler import DeviceSampler
@@ -294,6 +294,7 @@ def _multi_gpu_worker(rank, world, args, n_ent, n_rel, edges, port, valid=None, 
             name = args.dataset + "_" + args.model_name
             np.save(os.path.join(args.save_path, name + "_entity.npy"), ent.cpu().numpy())
             np.save(os.path.join(args.save_path, name + "_relation.npy"), trainer.rel_emb.cpu().numpy())
+            save_config(args)
     dist.barrier()
     dist.destroy_process_group()
 

@@ -22,6 +22,11 @@ def save_model(args, model, emap_file=None, rmap_file=None):
     os.makedirs(args.save_path, exist_ok=True)
     print("Save model to {}".format(args.save_path))
     model.save_emb(args.save_path, args.dataset)
+    save_config(args, emap_file, rmap_file)
+
+
+def save_config(args, emap_file=None, rmap_file=None):
+    """config.json of a checkpoint: the parsed arguments and the mapping files (utils.py:35-49)."""
     conf = dict(vars(args))
     conf.update({"emp_file": emap_file, "rmap_file": rmap_file})
     with open(os.path.join(args.save_path, "config.json"), "w") as f:

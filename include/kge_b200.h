@@ -265,6 +265,22 @@ KGE_API int kge_rank_count(kge_handle_t h, const float* S, int64_t ld, int64_t Q
 KGE_API int kge_rank_finish(kge_handle_t h, const int64_t* cnt, int64_t Q, int64_t* rank_out, double* acc,
                             void* stream);
 
+/* --- running top-K lists over score tiles (link prediction, ScoreInfer.topK of models/infer.py) ----------------------
+ * Merges score tile S [Q, ld] (N columns used) into G running lists of K entries:
+ *   row q feeds list g = qgroup[q] (0 <= g < G); the rows of one list are consecutive within a call
+ *   element (q, j) has key = qoff[q] + (cbase + j) * cstride (qoff >= 0, cbase >= 0, cstride >= 1); keys are distinct
+ *   top_score [G, K], top_key [G, K]: caller-owned device arrays, initialised once to -inf / -1 (empty slots)
+ * After the call every list holds the K best of (itself U the tile's elements of its rows) in the strict order
+ * score descending, then key ascending; fewer than K elements seen leaves trailing -inf / -1 slots.  A NaN score never
+ * enters, a -inf one does.  The result is the host sort of the same fp32 scores, bit for bit, whatever the launch
+ * geometry or timing.  1 <= K <= KGE_TOPK_MAX, else KGE_ERR_UNSUPPORTED (K > max) / KGE_ERR_INVALID_ARG (K < 1).
+ * Workspace: about Q * ceil(N / 4096) * (12 K + 4) + 4 G bytes, kept on the handle (it grows, synchronising the stream
+ * once, when a call needs more). */
+#define KGE_TOPK_MAX 1024
+KGE_API int kge_topk(kge_handle_t h, const float* S, int64_t ld, int64_t Q, int64_t N, const int64_t* qgroup,
+                     const int64_t* qoff, int64_t cbase, int64_t cstride, int32_t K, int64_t G, float* top_score,
+                     int64_t* top_key, void* stream);
+
 /* --- introspection (parity tests read the traced gradients the way the reference exposes
  *     `data.grad` of each trace entry, tensor_models.py:318) ---------------------------------- */
 typedef enum {
