@@ -120,6 +120,7 @@ struct kge_context {
   float* dump_v = nullptr;           // test hook (kge_debug_set_dump): coefficient matrices of the fused kernel
   Buffer negdeg_ids;                 // --neg_deg_sample: the augmented negative id list [C * (Cs + Ns)] of the last step
   Buffer topk_ws;                    // kge_topk: the select CTAs' survivors and the per-list bounds
+  Buffer sim_ws;                     // kge_sim_tile: TF32 hi/lo operands and row norms of the GEMM functions
   // kge_set_next_batch: rows of the next step staged by this step's fused kernels
   struct Prefetch {
     bool armed = false;              // a next batch is registered for the coming kge_step_fused_begin
@@ -436,7 +437,7 @@ KGE_API int kge_destroy(kge_handle_t h) {
   if (!h) return KGE_OK;
   DeviceGuard g(h->device);
   cudaDeviceSynchronize();
-  for (Buffer* b : {&h->arena, &h->dev_stage, &h->pin, &h->rel_dense, &h->negdeg_ids, &h->topk_ws, &h->pf.nc[0], &h->pf.nc[1],
+  for (Buffer* b : {&h->arena, &h->dev_stage, &h->pin, &h->rel_dense, &h->negdeg_ids, &h->topk_ws, &h->sim_ws, &h->pf.nc[0], &h->pf.nc[1],
                     &h->pf.bn[0], &h->pf.bn[1]})
     b->release();
   if (h->dev_log4) cudaFree(h->dev_log4);
@@ -640,6 +641,52 @@ KGE_API int kge_topk(kge_handle_t h, const float* S, int64_t ld, int64_t Q, int6
   topk_carve(p, h->topk_ws.p);
   KGE_CUDA_OK(cudaMemsetAsync(p.bound, 0, (size_t)G * sizeof(unsigned), st));
   launch_topk(lctx(h, stream), p);
+  KGE_CUDA_OK(cudaGetLastError());
+  return KGE_OK;
+}
+
+namespace {
+int check_sim_args(kge_handle_t h, int32_t sim, const float* left, const float* right, int32_t dim, const float* out) {
+  if (!h) return fail(KGE_ERR_INVALID_ARG, "handle is null");
+  if (sim < KGE_SIM_COSINE || sim > KGE_SIM_EXT_JACCARD) return fail(KGE_ERR_INVALID_ARG, "unknown similarity %d", (int)sim);
+  if (dim < 1 || dim > 160000) return fail(KGE_ERR_UNSUPPORTED, "dim=%d: kge_sim takes 1 <= dim <= 160000", (int)dim);
+  if (!left || !right || !out) return fail(KGE_ERR_INVALID_ARG, "null pointer");
+  return KGE_OK;
+}
+}  // namespace
+
+KGE_API int kge_sim_tile(kge_handle_t h, int32_t sim, const float* left, int64_t nL, const float* right, int64_t nR,
+                         int32_t dim, float* out, void* stream) {
+  if (nL < 0 || nR < 0) return fail(KGE_ERR_INVALID_ARG, "bad tile shape nL=%lld nR=%lld", (long long)nL, (long long)nR);
+  if (nL == 0 || nR == 0) return h ? KGE_OK : fail(KGE_ERR_INVALID_ARG, "handle is null");
+  if (int rc = check_sim_args(h, sim, left, right, dim, out)) return rc;
+  // grid rows (left tiles of 64) and columns (right tiles of 256) stay within the launch limits, and the TMA row
+  // coordinate of a slab, (32-column block) * n + row, within int32
+  const long long nblk = (dim + 31) / 32;
+  if (nL > 65535LL * 64 || nR > 65535LL * 256 || nblk * nL > 0x7fffffffLL || nblk * nR > 0x7fffffffLL)
+    return fail(KGE_ERR_INVALID_ARG, "tile too large: nL=%lld nR=%lld dim=%d", (long long)nL, (long long)nR, (int)dim);
+  DeviceGuard g(h->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (sim_uses_gemm(sim)) {
+    const size_t bytes = sim_workspace_bytes(nL, nR, dim);
+    if (h->sim_ws.bytes < bytes) {
+      const int rc = h->sim_ws.resize(bytes, st, "similarity workspace");
+      if (rc) return rc;
+    }
+  }
+  if (int rc = launch_sim_tile(lctx(h, stream), sim, left, nL, right, nR, dim, out, h->sim_ws.p)) return rc;
+  KGE_CUDA_OK(cudaGetLastError());
+  return KGE_OK;
+}
+
+KGE_API int kge_sim_pairs(kge_handle_t h, int32_t sim, const float* left, const float* right, int64_t n, int32_t dim,
+                          float* out, void* stream) {
+  if (n < 0) return fail(KGE_ERR_INVALID_ARG, "n=%lld < 0", (long long)n);
+  if (n == 0) return h ? KGE_OK : fail(KGE_ERR_INVALID_ARG, "handle is null");
+  if (int rc = check_sim_args(h, sim, left, right, dim, out)) return rc;
+  if ((n + 7) / 8 > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARG, "too many pairs: %lld", (long long)n);
+  DeviceGuard g(h->device);
+  launch_sim_pairs(lctx(h, stream), sim, left, right, n, dim, out);
   KGE_CUDA_OK(cudaGetLastError());
   return KGE_OK;
 }

@@ -463,6 +463,13 @@ size_t topk_workspace_bytes(long long Q, long long N, int K, long long G);
 void topk_carve(TopkParams& p, void* ws);
 void launch_topk(const LaunchCtx&, const TopkParams&);
 
+// embedding similarity tiles (kge_sim.cu)
+bool sim_uses_gemm(int sim);
+size_t sim_workspace_bytes(long long nL, long long nR, int dim);       // the GEMM functions' TF32 operands and norms
+int launch_sim_tile(const LaunchCtx&, int sim, const float* L, long long nL, const float* R, long long nR, int dim,
+                    float* S, void* ws);
+void launch_sim_pairs(const LaunchCtx&, int sim, const float* L, const float* R, long long n, int dim, float* out);
+
 // RESCAL-specific row kernels (kge_rescal.cu)
 int launch_rescal_prep(const LaunchCtx&, const StepParams&, const TableView& ent, const TableView& rel,
                        const BatchView&, const StepWs&);

@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("KGE_B200_LIB", os.path.join(os.path.dirname(_HERE), "
 
 KGE_MAX_SHARDS = 8
 KGE_TOPK_MAX = 1024
+SIM_IDS = {"cosine": 0, "l2": 1, "l1": 2, "dot": 3, "ext_jaccard": 4}       # kge_sim_t
 MODEL_IDS = {"TransE_l1": 0, "TransE": 1, "TransE_l2": 1, "DistMult": 2, "ComplEx": 3, "RESCAL": 4, "RotatE": 5}
 BUF_POS_SCORE, BUF_NEG_SCORE, BUF_NODE_GRAD, BUF_NEG_GRAD, BUF_REL_GRAD = range(5)
 
@@ -23,7 +24,7 @@ EXPORTS = ["kge_abi_version", "kge_last_error", "kge_create", "kge_destroy", "kg
            "kge_rel_grad_dense", "kge_rel_apply_dense", "kge_device_alloc", "kge_device_free", "kge_ipc_export",
            "kge_ipc_open", "kge_shard_alloc", "kge_shard_import", "kge_shard_free",
            "kge_set_next_batch", "kge_sampler_create", "kge_sampler_destroy", "kge_sampler_sample",
-           "kge_rank_count", "kge_rank_finish", "kge_topk"]
+           "kge_rank_count", "kge_rank_finish", "kge_topk", "kge_sim_tile", "kge_sim_pairs"]
 
 
 class KgeError(RuntimeError):
@@ -119,6 +120,8 @@ def load_library():
     lib.kge_rank_count.argtypes = [vp, vp, i64, i64, i64, vp, i64, vp, i64, vp, vp, P(Filter), vp, vp]
     lib.kge_rank_finish.argtypes = [vp, vp, i64, vp, vp, vp]
     lib.kge_topk.argtypes = [vp, vp, i64, i64, i64, vp, vp, i64, i64, i32, i64, vp, vp, vp]
+    lib.kge_sim_tile.argtypes = [vp, i32, vp, i64, vp, i64, i32, vp, vp]
+    lib.kge_sim_pairs.argtypes = [vp, i32, vp, vp, i64, i32, vp, vp]
     missing = [name for name in EXPORTS if not hasattr(lib, name)]
     if missing:
         raise KgeError("libkge_b200.so at %s lacks symbols %s (stale build?)" % (LIB_PATH, missing))

@@ -281,6 +281,25 @@ KGE_API int kge_topk(kge_handle_t h, const float* S, int64_t ld, int64_t Q, int6
                      const int64_t* qoff, int64_t cbase, int64_t cstride, int32_t K, int64_t G, float* top_score,
                      int64_t* top_key, void* stream);
 
+/* --- embedding similarity (dglke_emb_sim: EmbSimInfer of models/infer.py:216-343, the *_dist functions of
+ *     models/pytorch/tensor_models.py:59-100), fp32 rows x, y of `dim` floats ------------------------------------------
+ *   COSINE       x.y / (|x| |y|)                      (a zero row gives NaN, as in the reference)
+ *   L2           -|x - y|_2                           (difference form: x = y gives exactly -0.0)
+ *   L1           -|x - y|_1                           (likewise)
+ *   DOT          x.y
+ *   EXT_JACCARD  x.y / (|x|^2 + |y|^2 - x.y)          (|x|^2 is the square of the fp32 norm) */
+typedef enum { KGE_SIM_COSINE = 0, KGE_SIM_L2 = 1, KGE_SIM_L1 = 2, KGE_SIM_DOT = 3, KGE_SIM_EXT_JACCARD = 4 } kge_sim_t;
+/* out [nL, nR] (contiguous) = sim(left[i], right[j]); left [nL, dim], right [nR, dim] row-major (any alignment).
+ * DOT / COSINE / EXT_JACCARD: 3xTF32 tensor-core GEMM with the function applied to the accumulator; L1 / L2: fp32
+ * CUDA-core tiles.  1 <= dim <= 160000 (a RESCAL relation row at hidden 400).  The GEMM functions keep TF32 copies of
+ * both blocks on the handle: about 8 (nL + nR) ceil(dim / 32) * 32 bytes (it grows, synchronising the stream once, when
+ * a call needs more). */
+KGE_API int kge_sim_tile(kge_handle_t h, int32_t sim, const float* left, int64_t nL, const float* right, int64_t nR,
+                         int32_t dim, float* out, void* stream);
+/* out [n] = sim(left[i], right[i]) (the reference's pw=True) */
+KGE_API int kge_sim_pairs(kge_handle_t h, int32_t sim, const float* left, const float* right, int64_t n, int32_t dim,
+                          float* out, void* stream);
+
 /* --- introspection (parity tests read the traced gradients the way the reference exposes
  *     `data.grad` of each trace entry, tensor_models.py:318) ---------------------------------- */
 typedef enum {
